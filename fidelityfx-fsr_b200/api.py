@@ -245,6 +245,14 @@ class HostContext:
             ctypes.c_void_p(out_dev.data_ptr()), out_dev.stride(0) * out_dev.element_size(),
             ctypes.c_float(sharpness), flags, _stream(stream)))
 
+    def upscale_render(self, in_dev, render_w, render_h, out_dev, sharpness=0.25, flags=0, stream=None):
+        """One frame rendered at render_w x render_h (dynamic resolution): the top-left render region of `in_dev`, upscaled to the
+        context's output size with constants rebuilt from this frame's render size."""
+        _lib.check(_lib.lib().fsr1_context_upscale_render(
+            self._h, ctypes.c_void_p(in_dev.data_ptr()), in_dev.stride(0) * in_dev.element_size(), render_w, render_h,
+            ctypes.c_void_p(out_dev.data_ptr()), out_dev.stride(0) * out_dev.element_size(),
+            ctypes.c_float(sharpness), flags, _stream(stream)))
+
     def close(self):
         if self._h:
             _lib.lib().fsr1_context_destroy(self._h)

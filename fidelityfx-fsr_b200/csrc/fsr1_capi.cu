@@ -429,6 +429,7 @@ static int context_run(fsr1_context* c, void* in_dev, uint64_t in_pitch, void* o
 int fsr1_context_upscale_render(fsr1_context* c, const void* in_dev, uint64_t in_pitch, uint32_t render_w, uint32_t render_h,
                                 void* out_dev, uint64_t out_pitch, float sharpness, uint32_t flags, void* stream) {
   if (!c || !in_dev || !out_dev || !render_w || !render_h) return FSR1_ERR_INVALID_ARGUMENT;
+  if (render_w > c->in_w || render_h > c->in_h) return FSR1_ERR_INVALID_ARGUMENT;  // would read past the caller's input
   return context_run(c, const_cast<void*>(in_dev), in_pitch, out_dev, out_pitch, sharpness, flags, stream, render_w, render_h);
 }
 

@@ -70,8 +70,14 @@ class FSR_Filter:
         flags = self.flags | (api.FLAG_OUTPUT_SQUARE if hdr else 0)
         if self._intermediary is None or self._display != (displayWidth, displayHeight):
             raise api.Fsr1Error("call OnCreateWindowSizeDependentResources for this display size first")
-        econ = api.easu_con(pState.renderWidth, pState.renderHeight, pState.renderWidth, pState.renderHeight,
-                            displayWidth, displayHeight)
+        rw, rh = int(pState.renderWidth), int(pState.renderHeight)
+        if rw <= 0 or rh <= 0 or rw > inputTexture.shape[1] or rh > inputTexture.shape[0]:
+            raise api.Fsr1Error("render size %dx%d does not fit the %dx%d input texture"
+                                % (rw, rh, inputTexture.shape[1], inputTexture.shape[0]))
+        # the constants describe an input of exactly the render size: taps clamp at the render region's edge, so only that
+        # region is described (as fsr_filter.hpp does through fsr1_context_upscale_render)
+        inputTexture = inputTexture[:rh, :rw]
+        econ = api.easu_con(rw, rh, rw, rh, displayWidth, displayHeight)
         if pState.bUseRcas:
             rcon = api.rcas_con(pState.rcasAttenuation)
             api.upscale(inputTexture, self._intermediary, outputTexture, econ, rcon, flags=flags, stream=stream)

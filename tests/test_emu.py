@@ -11,6 +11,7 @@ import pytest
 
 import fsr1_b200 as F
 import oracle_lib as ol
+from easu_checks import assert_within_cell_bounds
 
 PROD = 12   # the production 2x kernel's number in the emulator harness (emu_easu.cpp)
 EMU_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu")
@@ -25,10 +26,10 @@ def emu_lib():
     return _lib
 
 
-def emu_easu(variant, src_h, ow, oh, y0=0, y1=None, ctas=3):
+def emu_easu(variant, src_h, ow, oh, y0=0, y1=None, ctas=3, con=None):
     ih, iw = src_h.shape[:2]
     y1 = oh if y1 is None else y1
-    con = (ctypes.c_uint32 * 16)(*ol.easu_con(iw, ih, ow, oh))
+    con = (ctypes.c_uint32 * 16)(*(con or ol.easu_con(iw, ih, ow, oh)))
     src = np.ascontiguousarray(src_h.view(np.uint16))
     out = np.zeros((oh, ow, 4), np.uint16)
     rc = emu_lib().emu_easu_h_quad2x(variant, ctypes.c_void_p(src.ctypes.data), iw, ih, ctypes.c_longlong(src.strides[0]),
@@ -60,10 +61,10 @@ def test_emulated_row_range_only_touches_its_rows():
     assert not part[:19].view(np.uint16).any() and not part[53:].view(np.uint16).any()
 
 
-def emu_easu_pairs(src_h, ow, oh, y0=0, y1=None, ctas=2, variant=1):
+def emu_easu_pairs(src_h, ow, oh, y0=0, y1=None, ctas=2, variant=1, con=None):
     ih, iw = src_h.shape[:2]
     y1 = oh if y1 is None else y1
-    con = (ctypes.c_uint32 * 16)(*ol.easu_con(iw, ih, ow, oh))
+    con = (ctypes.c_uint32 * 16)(*(con or ol.easu_con(iw, ih, ow, oh)))
     src = np.ascontiguousarray(src_h.view(np.uint16))
     out = np.zeros((oh, ow, 4), np.uint16)
     rc = emu_lib().emu_easu_h_pairs(variant, ctypes.c_void_p(src.ctypes.data), iw, ih, ctypes.c_longlong(src.strides[0]),
@@ -311,33 +312,87 @@ def test_emulated_fused_kernel_is_bit_identical_to_the_two_kernel_path(size, cta
             assert not out[:y0].any() and not out[y1:].any()
 
 
+def emu_easu_f32_pairs(src, ow, oh, con, y0=0, y1=None, ctas=2):
+    """easu_f32_pairs_kernel on a float32 image, or on a float16 image with fp32 arithmetic (FSR1_FLAG_PRECISE)."""
+    ih, iw = src.shape[:2]
+    y1 = oh if y1 is None else y1
+    half_storage = src.dtype == np.float16
+    s = np.ascontiguousarray(src.view(np.uint16) if half_storage else src)
+    out = np.zeros((oh, ow, 4), np.uint16 if half_storage else np.float32)
+    rc = emu_lib().emu_easu_f32_pairs(1 if half_storage else 0, ctypes.c_void_p(s.ctypes.data), iw, ih, ctypes.c_longlong(s.strides[0]),
+                                      ctypes.c_void_p(out.ctypes.data), ow, oh, ctypes.c_longlong(out.strides[0]),
+                                      (ctypes.c_uint32 * 16)(*con), y0, y1, ctas)
+    assert rc == 0
+    return out.view(np.float16) if half_storage else out
+
+
 @pytest.mark.parametrize("shape", [(96, 54, 144, 81), (96, 54, 125, 70), (64, 64, 64, 64), (50, 20, 65, 26), (33, 17, 57, 31), (96, 54, 192, 81)])
 @pytest.mark.parametrize("half_storage", [0, 1])
-def test_emulated_any_scale_fp32_kernel(shape, half_storage):
+def test_emulated_any_scale_fp32_kernel(shape, half_storage, con=None):
     """easu_f32_pairs_kernel: RGBA32F images (or fp32 arithmetic on RGBA16F storage, FSR1_FLAG_PRECISE) at scales other than 2x —
     the structure of the fp16 any-scale kernel with pairwise fp32 tap weights; within 1e-5 of the oracle (fp32 storage) / one
     rounding to half (fp16 storage), row ranges included."""
     iw, ih, ow, oh = shape
-    con = (ctypes.c_uint32 * 16)(*ol.easu_con(iw, ih, ow, oh))
+    con = con or ol.easu_con(iw, ih, ow, oh)
     for gen in (F.uniform, F.structured):
-        src32 = gen(iw, ih, 31)
+        src = gen(iw, ih, 31)
         if half_storage:
-            src = np.ascontiguousarray(F.to_half(src32).view(np.uint16))
-            want = ol.easu(src.view(np.float16).astype(np.float32), ow, oh)
-            out = np.zeros((oh, ow, 4), np.uint16)
-        else:
-            src = np.ascontiguousarray(src32)
-            want = ol.easu(src, ow, oh)
-            out = np.zeros((oh, ow, 4), np.float32)
-        def run(y0, y1, ctas, dst):
-            rc = emu_lib().emu_easu_f32_pairs(half_storage, ctypes.c_void_p(src.ctypes.data), iw, ih, ctypes.c_longlong(src.strides[0]),
-                                              ctypes.c_void_p(dst.ctypes.data), ow, oh, ctypes.c_longlong(dst.strides[0]), con, y0, y1, ctas)
-            assert rc == 0
-        run(0, oh, 2, out)
-        got = out.view(np.float16).astype(np.float32) if half_storage else out
+            src = F.to_half(src)
+        want = ol.easu(src.astype(np.float32), ow, oh, con)
+        out = emu_easu_f32_pairs(src, ow, oh, con)
+        got = out.astype(np.float32)
         assert np.abs(got - want)[..., :3].max() <= (6e-4 if half_storage else 1e-5)
         assert (got[..., 3] == 1.0).all()
-        part = np.zeros_like(out)
+        assert_within_cell_bounds(out, src, con, what=(shape, half_storage))
         y0, y1 = oh // 3, 2 * oh // 3 + 1
-        run(y0, y1, 1, part)
+        part = emu_easu_f32_pairs(src, ow, oh, con, y0=y0, y1=y1, ctas=1)
         assert np.array_equal(part[y0:y1], out[y0:y1]) and not part[:y0].any() and not part[y1:].any()
+
+
+# The geometry cases of tests/test_gpu_parity.py (GEOMETRY) at emulator size: viewports smaller than the resource, FsrEasuConOffset,
+# non-uniform and extreme scales and "almost 2x" sizes.  Outputs span several 64x32 tiles, so one or two CTAs walk more than
+# one tile (prefetch into the other buffer, mbarrier parity flip).  One axis downscaled selects the direct kernel, which the
+# emulator does not build; the GPU suite covers it.
+# id: (resource w, h, viewport w, h, offset or None, output w, h)
+EMU_GEOMETRY = {
+    "2x_viewport": (96, 40, 48, 20, None, 96, 40),
+    "offset": (96, 40, 64, 26, (8, 4), 96, 39),
+    "viewport_at_resource_edge": (96, 40, 48, 20, (48, 20), 96, 40),
+    "anisotropic_x2_y1.5": (48, 26, 48, 26, None, 96, 39),
+    "x1.5_y1": (64, 40, 64, 40, None, 96, 40),
+    "x1_y1.5": (96, 26, 96, 26, None, 96, 39),
+    "scale1": (96, 40, 96, 40, None, 96, 40),
+    "3x": (32, 13, 32, 13, None, 96, 39),
+    "4x": (24, 10, 24, 10, None, 96, 40),
+    "almost_2x_41x47": (41, 47, 41, 47, None, 82, 94),
+}
+
+
+@pytest.mark.parametrize("case", list(EMU_GEOMETRY))
+def test_emulated_geometry_against_oracle(case):
+    """The tiled EASU kernels at this geometry against the oracle reading the whole resource with the same constants: the
+    emulator tolerances, the de-ringing bound (no tolerance), one CTA == several CTAs and row ranges == the whole frame."""
+    iw, ih, vw, vh, off, ow, oh = EMU_GEOMETRY[case]
+    con = ol.easu_con(iw, ih, ow, oh, vw, vh, off=off)
+    quad = con[:4] == [0x3F000000, 0x3F000000, 0xBE800000, 0xBE800000]
+    y0, y1 = oh // 3, 2 * oh // 3 + 1
+    for gen in (F.uniform, F.structured):
+        src32 = gen(iw, ih, 77)
+        src = F.to_half(src32)
+        want = ol.easu(src.astype(np.float32), ow, oh, con)
+        run = (lambda **kw: emu_easu(PROD, src, ow, oh, con=con, **kw)) if quad else (lambda **kw: emu_easu_pairs(src, ow, oh, con=con, **kw))
+        got = run(ctas=2)
+        assert np.abs(got.astype(np.float32) - want)[..., :3].max() <= 5e-3, (case, gen.__name__)
+        assert_within_cell_bounds(got, src, con, what=(case, gen.__name__, "f16"))
+        assert np.array_equal(run(ctas=1).view(np.uint16), got.view(np.uint16)), (case, "one CTA")
+        part = run(y0=y0, y1=y1, ctas=1)
+        assert np.array_equal(part[y0:y1].view(np.uint16), got[y0:y1].view(np.uint16)), (case, "rows")
+        if quad:
+            continue
+        for s, tol in ((src32, 1e-5), (src, 6e-4)):                      # RGBA32F, and fp32 arithmetic on RGBA16F storage
+            got = emu_easu_f32_pairs(s, ow, oh, con, ctas=2)
+            assert np.abs(got.astype(np.float32) - ol.easu(s.astype(np.float32), ow, oh, con))[..., :3].max() <= tol, (case, s.dtype)
+            assert_within_cell_bounds(got, s, con, what=(case, gen.__name__, str(s.dtype)))
+            assert np.array_equal(emu_easu_f32_pairs(s, ow, oh, con, ctas=1), got), (case, s.dtype, "one CTA")
+            part = emu_easu_f32_pairs(s, ow, oh, con, y0=y0, y1=y1, ctas=1)
+            assert np.array_equal(part[y0:y1], got[y0:y1]), (case, s.dtype, "rows")

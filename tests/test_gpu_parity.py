@@ -13,6 +13,7 @@ import torch
 
 import fsr1_b200 as F
 import oracle_lib as ol
+from easu_checks import assert_within_cell_bounds, expected_easu_kernel
 
 pytestmark = pytest.mark.gpu
 api = F.api
@@ -21,24 +22,40 @@ G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "
 GSIZES = {"x2.0": (64, 36), "x1.5": (48, 27), "x1.3": (41, 23), "x1.0": (32, 18), "x2.0x1.5": (64, 27)}
 
 
+def _padded(w, itemsize):
+    """Row length in pixels of a 16-byte multiple (and even, as the fp16 / fp32 images always were)."""
+    per = max(2, 16 // (4 * itemsize))
+    return -(-w // per) * per
+
+
 def dev(a):
     """Upload [H,W,4]; rows are padded to a 16-byte multiple (like any real texture allocation) so that the
     production kernels apply to odd widths too; the returned tensor is the [H,W,4] view."""
     h, w = a.shape[:2]
-    wp = (w + 1) & ~1
-    t = torch.zeros((h, wp, 4), dtype=torch.from_numpy(a[:0]).dtype, device="cuda")
+    t = torch.zeros((h, _padded(w, a.itemsize), 4), dtype=torch.from_numpy(a[:0]).dtype, device="cuda")
     t[:, :w] = torch.from_numpy(np.ascontiguousarray(a)).cuda()
     return t[:, :w]
 
 
 def empty_like_image(h, w, dtype):
-    return torch.zeros((h, (w + 1) & ~1, 4), dtype=dtype, device="cuda")[:, :w]
+    return torch.zeros((h, _padded(w, torch.empty(0, dtype=dtype).element_size()), 4), dtype=dtype, device="cuda")[:, :w]
+
+
+def fmt_of(a):
+    return {np.dtype(np.float16): api.FORMAT_RGBA16F, np.dtype(np.float32): api.FORMAT_RGBA32F,
+            np.dtype(np.uint8): api.FORMAT_RGBA8_UNORM}[np.dtype(a.dtype)]
+
+
+def assert_kernel(con, src, flags=0):
+    """The kernel family of the last launch is the one the launchers' selection rule gives for these constants."""
+    want = expected_easu_kernel(con, fmt_of(src), flags)
+    assert api.last_kernel().startswith(want), (api.last_kernel(), want)
 
 
 def gpu_easu(src, ow, oh, flags=0, con=None, y0=0, y1=0):
     ih, iw = src.shape[:2]
     con = con or api.easu_con(iw, ih, iw, ih, ow, oh)
-    out = empty_like_image(oh, ow, torch.float16 if src.dtype == np.float16 else torch.float32)
+    out = empty_like_image(oh, ow, torch.from_numpy(src[:0]).dtype)
     api.easu(dev(src), out, con, y0=y0, y1=y1, flags=flags)
     torch.cuda.synchronize()
     return out.cpu().numpy()
@@ -51,8 +68,9 @@ def gpu_rcas(src, sharp, flags=0, y0=0, y1=0):
     return out.cpu().numpy()
 
 
+# (41, 47, 82, 94): twice the size, but fp32 41 * rcp(82) = 0.49999997, so not the 2x kernels
 SHAPES = [(96, 54, 192, 108), (96, 54, 144, 81), (96, 54, 125, 70), (33, 17, 57, 31), (7, 5, 14, 10), (64, 64, 64, 64),
-          (3, 3, 9, 9), (1, 1, 4, 4), (50, 20, 65, 26), (130, 70, 259, 141), (200, 40, 401, 79)]
+          (3, 3, 9, 9), (1, 1, 4, 4), (50, 20, 65, 26), (130, 70, 259, 141), (200, 40, 401, 79), (41, 47, 82, 94)]
 
 
 @pytest.mark.parametrize("shape", SHAPES)
@@ -77,8 +95,8 @@ def test_fp32_default_within_1e5(shape, gen):
     src = getattr(F, gen)(iw, ih, 32)
     want = ol.easu(src, ow, oh)
     got = gpu_easu(src, ow, oh)
-    # a TMA-tiled kernel at every scale: the quad kernel at exactly 2x, the vertical-pair kernel otherwise (never easu_direct)
-    assert api.last_kernel().startswith("easu_f32_quad2x" if (2 * iw, 2 * ih) == (ow, oh) else "easu_f32_vpairs"), api.last_kernel()
+    # a TMA-tiled kernel at every upscale: the quad kernel at exactly 2x, the vertical-pair kernel otherwise (never easu_direct)
+    assert_kernel(api.easu_con(iw, ih, iw, ih, ow, oh), src)
     assert np.abs(got - want).max() <= TOL32
     alt = gpu_easu(src, ow, oh, api.FLAG_FORCE_DIRECT)
     assert api.last_kernel().startswith("easu_direct<f32,fast") and np.abs(alt - want).max() <= TOL32
@@ -95,7 +113,7 @@ def test_fp16_kernels_within_1e2_of_fp32_oracle(shape, gen):
     src = F.to_half(getattr(F, gen)(iw, ih, 33))
     want = ol.easu(src.astype(np.float32), ow, oh)       # fp32 algorithm on the quantised input
     got = gpu_easu(src, ow, oh)
-    assert api.last_kernel().startswith("easu_h_"), api.last_kernel()
+    assert_kernel(api.easu_con(iw, ih, iw, ih, ow, oh), src)
     assert got.dtype == np.float16 and np.all(got[..., 3] == 1.0)
     assert np.abs(got.astype(np.float32) - want).max() <= TOL16
     # the fp32-math / fp16-storage fallback kernel is held to the same bound
@@ -237,7 +255,7 @@ def test_precise_flag_fp32_math_on_fp16_storage():
         src = F.to_half(getattr(F, gen)(iw, ih, 35))
         want = ol.easu(src.astype(np.float32), ow, oh)
         got = gpu_easu(src, ow, oh, api.FLAG_PRECISE)
-        assert api.last_kernel().startswith("easu_h16io_f32math"), api.last_kernel()
+        assert_kernel(api.easu_con(iw, ih, iw, ih, ow, oh), src, api.FLAG_PRECISE)
         assert np.abs(got.astype(np.float32) - want).max() <= 6e-4      # half ulp at 1.0 is 4.9e-4
         assert np.all(got[..., 3] == 1.0)
         mid = gpu_rcas(got, 0.25)
@@ -245,7 +263,7 @@ def test_precise_flag_fp32_math_on_fp16_storage():
         for (ow2, oh2) in ((300, 180), (261, 157)):                       # 1.5x and ~1.3x: the any-scale fp32-math kernel
             want2 = ol.easu(src.astype(np.float32), ow2, oh2)
             got2 = gpu_easu(src, ow2, oh2, api.FLAG_PRECISE)
-            assert api.last_kernel().startswith("easu_h16io_f32math_vpairs"), api.last_kernel()
+            assert_kernel(api.easu_con(iw, ih, iw, ih, ow2, oh2), src, api.FLAG_PRECISE)
             assert np.abs(got2.astype(np.float32) - want2).max() <= 6e-4
 
 
@@ -331,9 +349,14 @@ def test_slabs_compose(dt, shape):
     """Row windows (the multi-GPU slabs) give exactly the bytes of the whole-frame run — for the 2x kernels, the
     generic kernel (1.5x, 1.3x) and the direct kernels alike."""
     iw, ih, ow, oh = shape
-    src = F.uniform(iw, ih, 13).astype(dt)
-    tdt = torch.float16 if dt == np.float16 else torch.float32
-    econ, rcon = api.easu_con(iw, ih, iw, ih, ow, oh), api.rcas_con(0.25)
+    check_slabs_compose(F.uniform(iw, ih, 13).astype(dt), ow, oh, api.easu_con(iw, ih, iw, ih, ow, oh))
+
+
+def check_slabs_compose(src, ow, oh, econ):
+    """Three row slabs, each with the input window SlabPlan gives it, reproduce the bytes of the whole-frame upscale."""
+    ih = src.shape[0]
+    tdt = torch.from_numpy(src[:0]).dtype
+    rcon = api.rcas_con(0.25)
     full_in = dev(src)
     tmp = empty_like_image(oh, ow, tdt)
     whole = empty_like_image(oh, ow, tdt)
@@ -448,13 +471,7 @@ def test_full_size_1080p_to_4k_against_oracle():
     assert np.abs(out.cpu().numpy().astype(np.float32) - r_want).max() <= TOL16
     e2e_check(out.cpu().numpy(), ol.rcas(e_want, ol.rcas_con(0.25)), "1080p->4K structured")
     # size-independent property: the de-ringing clamp — every EASU output lies within the min/max of its 2x2 cell
-    pad = np.pad(src.astype(np.float32), ((2, 2), (2, 2), (0, 0)), mode="edge")
-    ys, xs = np.arange(oh), np.arange(ow)
-    fy = np.floor((ys + 0.5) * 0.5 - 0.5).astype(int) + 2
-    fx = np.floor((xs + 0.5) * 0.5 - 0.5).astype(int) + 2
-    quad = np.stack([pad[fy][:, fx], pad[fy][:, fx + 1], pad[fy + 1][:, fx], pad[fy + 1][:, fx + 1]])
-    g = e_got.astype(np.float32)[..., :3]
-    assert np.all(g >= quad.min(0)[..., :3]) and np.all(g <= quad.max(0)[..., :3])
+    assert_within_cell_bounds(e_got, src, econ, what="1080p->4K")
 
 
 # ---- BASELINE.json configs at their own size (every pixel against the oracle) ----------------------------------------
@@ -667,3 +684,209 @@ def test_fused_kernel_full_size_1080p_to_4k(gen):
     torch.cuda.synchronize()
     assert torch.equal(got, want)
     e2e_check(got.cpu().numpy(), ol.rcas(ol.easu(src.astype(np.float32), ow, oh), ol.rcas_con(0.25)), ("fused", gen))
+
+
+# ---- geometry: viewports, offsets, non-uniform and extreme scales, multi-wave launches ------------------------------------
+# Each output is about 1080p or larger, so every persistent kernel walks more tiles than it has CTAs (prefetch into the other
+# buffer, mbarrier parity flip, tile walk after the first tile).  The kernel family is predicted from the constant block.
+# id: (resource w, h, viewport w, h, offset or None, output w, h)
+GEOMETRY = {
+    "2x_viewport": (1920, 1080, 960, 540, None, 1920, 1080),
+    "offset_1280x720_at_16_8": (1920, 1080, 1280, 720, (16, 8), 2560, 1440),
+    "viewport_at_resource_edge": (1920, 1080, 960, 540, (960, 540), 1920, 1080),
+    "anisotropic_x2_y1.5": (1920, 1080, 1920, 1080, None, 3840, 1620),
+    "anisotropic_x1.34_y1.33": (2560, 1080, 2560, 1080, None, 3440, 1440),
+    "x1.5_y1": (1280, 1080, 1280, 1080, None, 1920, 1080),
+    "x1_y1.5": (1920, 720, 1920, 720, None, 1920, 1080),
+    "scale1": (1920, 1080, 1920, 1080, None, 1920, 1080),
+    "3x": (640, 360, 640, 360, None, 1920, 1080),
+    "4x": (480, 270, 480, 270, None, 1920, 1080),
+    "y_downscaled": (1920, 1080, 1920, 1080, None, 2880, 900),
+    "almost_2x_949x564": (949, 564, 949, 564, None, 1898, 1128),
+    "almost_2x_41x47": (41, 47, 41, 47, None, 82, 94),
+}
+
+
+def geometry_con(iw, ih, vw, vh, off, ow, oh):
+    if off is None:
+        return api.easu_con(vw, vh, iw, ih, ow, oh)
+    return api.easu_con_offset(vw, vh, iw, ih, ow, oh, float(off[0]), float(off[1]))
+
+
+def report(case, what, got, want):
+    """Max / mean abs error of one kernel against its oracle, printed with the kernel that ran (pytest -s shows it)."""
+    d = np.abs(got[..., :3].astype(np.float64) - want[..., :3].astype(np.float64))
+    print("EASU %-28s %-16s %-52s max %.3g mean %.3g" % (case, what, api.last_kernel(), d.max(), d.mean()))
+    return d
+
+
+@pytest.mark.parametrize("case", list(GEOMETRY))
+def test_geometry_against_oracle(case):
+    """Every format's EASU kernel at this geometry against the oracle reading the whole resource with the same constants: the
+    suite's contract per format, the de-ringing bound, the kernel family the constants select, and row slabs that compose."""
+    iw, ih, vw, vh, off, ow, oh = GEOMETRY[case]
+    con = geometry_con(iw, ih, vw, vh, off, ow, oh)
+    src = F.uniform(iw, ih, 4000 + iw + ih)
+    src_h = F.to_half(src)
+    f_h = src_h.astype(np.float32)
+    raw = np.floor(src * 255.0 + 0.5).astype(np.uint8)
+    fin = raw.astype(np.float32) / np.float32(255.0)
+
+    want = ol.easu(src, ow, oh, con)
+    got = gpu_easu(src, ow, oh, con=con)                                     # RGBA32F, default
+    assert_kernel(con, src)
+    assert report(case, "f32", got, want).max() <= TOL32
+    assert_within_cell_bounds(got, src, con, what=(case, "f32"))
+    got = gpu_easu(src, ow, oh, api.FLAG_EXACT, con=con)                    # RGBA32F, EXACT: bit for bit
+    assert_kernel(con, src, api.FLAG_EXACT)
+    report(case, "f32 exact", got, want)
+    assert np.array_equal(got.view(np.uint32), want.view(np.uint32))
+    assert_within_cell_bounds(got, src, con, what=(case, "f32 exact"))
+
+    want = ol.easu(f_h, ow, oh, con)                                         # fp32 algorithm on the half input
+    got = gpu_easu(src_h, ow, oh, con=con)                                   # RGBA16F, default
+    assert_kernel(con, src_h)
+    assert report(case, "f16", got, want).max() <= TOL16
+    assert_within_cell_bounds(got, src_h, con, what=(case, "f16"))
+    got = gpu_easu(src_h, ow, oh, api.FLAG_PRECISE, con=con)                # RGBA16F, PRECISE
+    assert_kernel(con, src_h, api.FLAG_PRECISE)
+    assert report(case, "f16 precise", got, want).max() <= 6e-4
+    assert_within_cell_bounds(got, src_h, con, what=(case, "f16 precise"))
+    got = gpu_easu(src_h, ow, oh, api.FLAG_H_REFERENCE, con=con)            # RGBA16F, the literal FsrEasuH: bit for bit
+    assert_kernel(con, src_h, api.FLAG_H_REFERENCE)
+    want_h = ol.easu(src_h, ow, oh, con)
+    report(case, "f16 href", got, want_h)
+    assert np.array_equal(got.view(np.uint16), want_h.view(np.uint16))
+    assert_within_cell_bounds(got, src_h, con, what=(case, "f16 href"))
+
+    want8 = _q(ol.easu(fin, ow, oh, con)[..., :3], 8)                        # R8G8B8A8: code values
+    got = gpu_easu(raw, ow, oh, con=con)
+    assert_kernel(con, raw)
+    assert report(case, "u8 (codes)", got, want8).max() <= 1
+    assert_within_cell_bounds(got, raw, con, what=(case, "u8"))
+
+    econ_is_2x = expected_easu_kernel(con, api.FORMAT_RGBA16F) == "easu_h_quad2x"
+    if econ_is_2x:                                                           # fused == two kernels, bit for bit
+        din, rcon = dev(src_h), api.rcas_con(0.25)
+        tmp, two = empty_like_image(oh, ow, torch.float16), empty_like_image(oh, ow, torch.float16)
+        api.upscale(din, tmp, two, con, rcon)
+        fused = empty_like_image(oh, ow, torch.float16)
+        api.upscale(din, tmp, fused, con, rcon, flags=api.FLAG_FUSED)
+        assert api.last_kernel().startswith("fused_easu_rcas_h"), api.last_kernel()
+        torch.cuda.synchronize()
+        assert torch.equal(fused, two)
+    for s in (src_h, src, raw):
+        check_slabs_compose(s, ow, oh, con)
+
+
+@pytest.mark.parametrize("gen", ["uniform", "structured"])
+def test_full_size_fp32_and_precise_1440p_to_4k(gen):
+    """The fp32 any-scale kernels (the slow fallback at the Quality preset) at full size: 1020 tiles against at most 2 x 132 CTAs."""
+    iw, ih, ow, oh = 2560, 1440, 3840, 2160
+    src = getattr(F, gen)(iw, ih, 12345)
+    econ, rcon = api.easu_con(iw, ih, iw, ih, ow, oh), api.rcas_con(0.25)
+    tmp = torch.zeros((oh, ow, 4), dtype=torch.float32, device="cuda")
+    out = torch.zeros_like(tmp)
+    api.upscale(dev(src), tmp, out, econ, rcon)
+    torch.cuda.synchronize()
+    e_want = ol.easu(src, ow, oh)
+    e_got = tmp.cpu().numpy()
+    api.easu(dev(src), tmp, econ)
+    assert_kernel(econ, src)
+    assert report("1440p->4K " + gen, "f32", e_got, e_want).max() <= TOL32
+    assert_within_cell_bounds(e_got, src, econ, what="f32 1440p->4K")
+    got = out.cpu().numpy()
+    assert np.abs(got - ol.rcas(e_got, rcon)).max() <= TOL32                  # RCAS on the kernel's own intermediate
+    assert np.abs(got - ol.rcas(e_want, rcon))[..., :3].max() <= 5e-5         # end to end
+    src_h = F.to_half(src)
+    got_h = gpu_easu(src_h, ow, oh, api.FLAG_PRECISE)
+    assert_kernel(econ, src_h, api.FLAG_PRECISE)
+    assert report("1440p->4K " + gen, "f16 precise", got_h, ol.easu(src_h.astype(np.float32), ow, oh)).max() <= 6e-4
+    assert_within_cell_bounds(got_h, src_h, econ, what="precise 1440p->4K")
+
+
+# ---- dynamic resolution: one context, the render size changing from frame to frame --------------------------------------
+SEQUENCE = [(960, 540), (1280, 720), (1129, 635), (1476, 830), (1920, 1080), (640, 360), (949, 540), (960, 540)]
+
+
+@pytest.mark.parametrize("fmt,flags", [("f16", 0), ("f32", 0), ("u8", 0), ("f16", api.FLAG_FUSED), ("f16", api.FLAG_PRECISE)],
+                         ids=["f16", "f32", "u8", "f16-fused", "f16-precise"])
+def test_dynamic_resolution_frame_sequence(fmt, flags):
+    """fsr1_context_upscale_render (the path of the C++ FSR_Filter) and the Python FSR_Filter on a 1920x1080 buffer whose top-left
+    render region changes size every frame, so the kernels move between the quad, vertical-pair and direct families.  Every texel
+    outside the render region holds a sentinel; a tap that reads it breaks the de-ringing bound.  Each frame equals fsr1_upscale
+    on the cropped view, bit for bit, and is held to the format's contract against the oracle."""
+    W, H = 1920, 1080
+    dt = {"f16": np.float16, "f32": np.float32, "u8": np.uint8}[fmt]
+    tdt = torch.from_numpy(np.zeros(0, dt)).dtype
+    fmt_id = {"f16": api.FORMAT_RGBA16F, "f32": api.FORMAT_RGBA32F, "u8": api.FORMAT_RGBA8_UNORM}[fmt]
+    sentinel = 255 if fmt == "u8" else 4.0
+    rcon = api.rcas_con(0.25)
+    ctx = api.HostContext(W, H, W, H, fmt_id)
+    flt = F.FSR_Filter()
+    flt.OnCreate(dtype=tdt)
+    flt.flags = flags
+    flt.OnCreateWindowSizeDependentResources(W, H, W, H)
+    buf = torch.full((H, W, 4), sentinel, dtype=tdt, device="cuda")
+    for i, (rw, rh) in enumerate(SEQUENCE):
+        f32 = F.uniform(rw, rh, 500 + i)
+        content = np.floor(f32 * 255.0 + 0.5).astype(np.uint8) if fmt == "u8" else f32.astype(dt)
+        buf.fill_(sentinel)
+        buf[:rh, :rw] = torch.from_numpy(content).cuda()
+        crop = buf[:rh, :rw]
+        con = api.easu_con(rw, rh, rw, rh, W, H)
+        out_ctx = torch.zeros((H, W, 4), dtype=tdt, device="cuda")
+        ctx.upscale_render(buf, rw, rh, out_ctx, 0.25, flags)
+        tmp, want = torch.zeros_like(out_ctx), torch.zeros_like(out_ctx)
+        api.upscale(crop, tmp, want, con, rcon, flags=flags)
+        if flags & api.FLAG_FUSED:
+            two_x = expected_easu_kernel(con, fmt_id) == "easu_h_quad2x"
+            assert api.last_kernel().startswith("fused_easu_rcas_h" if two_x else "rcas_h_packed"), (rw, rh, api.last_kernel())
+        out_flt = torch.zeros_like(out_ctx)
+        flt.Upscale(buf, out_flt, W, H, F.State(renderWidth=rw, renderHeight=rh, rcasAttenuation=0.25))
+        e_flags = flags & ~api.FLAG_FUSED
+        api.easu(crop, tmp, con, flags=e_flags)
+        assert_kernel(con, content, e_flags)
+        kernel = api.last_kernel()
+        torch.cuda.synchronize()
+        assert torch.equal(out_ctx, want), (rw, rh)
+        assert torch.equal(out_flt, out_ctx), (rw, rh)
+        e_got, got = tmp.cpu().numpy(), out_ctx.cpu().numpy()
+        what = "%dx%d %s flags=%d" % (rw, rh, fmt, flags)
+        assert_within_cell_bounds(e_got, content, con, what=what)
+        if fmt == "u8":
+            fin = content.astype(np.float32) / np.float32(255.0)
+            d = np.abs(e_got[..., :3].astype(np.int64) - _q(ol.easu(fin, W, H)[..., :3], 8).astype(np.int64))
+            mid = e_got.astype(np.float32) / np.float32(255.0)
+            r = np.abs(got[..., :3].astype(np.int64) - _q(ol.rcas(mid, rcon)[..., :3], 8).astype(np.int64))
+            print("frame %-24s %-52s EASU max %d codes mean %.3g; RCAS max %d codes" % (what, kernel, d.max(), d.mean(), r.max()))
+            assert d.max() <= 1 and r.max() <= 1, (what, int(d.max()), int(r.max()))
+            continue
+        e_want = ol.easu(content.astype(np.float32), W, H)
+        d = np.abs(e_got.astype(np.float32) - e_want)[..., :3]
+        print("frame %-24s %-52s EASU max %.3g mean %.3g" % (what, kernel, d.max(), d.mean()))
+        assert d.max() <= (TOL32 if fmt == "f32" else 6e-4 if flags & api.FLAG_PRECISE else TOL16), (what, d.max())
+        if fmt == "f32":
+            assert np.abs(got - ol.rcas(e_got, rcon)).max() <= TOL32, what
+            assert np.abs(got - ol.rcas(e_want, rcon))[..., :3].max() <= 5e-5, what
+        else:
+            assert np.abs(got.astype(np.float32) - ol.rcas(e_got.astype(np.float32), rcon))[..., :3].max() <= TOL16, what
+            if not flags & api.FLAG_PRECISE and W > 2.1 * rw:
+                # Not held end to end above 2x.  At 3x (640x360) the half-arithmetic EASU is within its own bounds (2.7e-3 of the
+                # oracle, inside every cell's texel range), but on that smooth 3x content RCAS amplifies EASU errors of at most
+                # 9e-4 around one pixel about 20x, to 1.9e-2, past the 1e-2 measured at 2x.  The CPU emulator, which runs the same
+                # device code, gives the same numbers.
+                continue
+            e2e_check(got, ol.rcas(e_want, rcon), what, tight=bool(flags & api.FLAG_PRECISE))
+    # a render size larger than the context's input is refused before anything is launched, even where the caller's buffer
+    # is large enough to read from
+    big = torch.zeros((H + 8, W + 16, 4), dtype=tdt, device="cuda")
+    n0 = api.launch_count()
+    for (rw, rh) in ((W + 16, H), (W, H + 8), (W + 16, H + 8)):
+        with pytest.raises(api.Fsr1Error):
+            ctx.upscale_render(big, rw, rh, out_ctx, 0.25, flags)
+        with pytest.raises(api.Fsr1Error):
+            flt.Upscale(buf, out_flt, W, H, F.State(renderWidth=rw, renderHeight=rh))
+    assert api.launch_count() == n0
+    ctx.close()
+    flt.OnDestroy()

@@ -3,8 +3,8 @@ production kernels' own device code, checked against the oracle.  GPU-free; minu
 
     python tools/emu_fuzz.py [seconds=300] [seed=1]
 
-Checks per case: 2x EASU (quad kernel) and any-scale EASU (vertical-pair kernel) within 5e-3 of the fp32 oracle, row range == the
-same rows of the full frame; packed RCAS within 4e-3, both out-of-image rules, options; fused kernel == two-kernel path bit for
+Checks per case: 2x EASU (quad kernel) and any-scale EASU (vertical-pair kernel, also on a viewport of the resource and at an
+offset, and within the de-ringing bound) within 5e-3 of the fp32 oracle, row range == the same rows of the full frame; packed RCAS within 4e-3, both out-of-image rules, options; fused kernel == two-kernel path bit for
 bit; the Hx2 kernels bit-identical to the half oracle."""
 import ctypes
 import os
@@ -20,6 +20,7 @@ import fsr1_b200 as F  # noqa: E402
 import oracle_lib as ol  # noqa: E402
 import test_emu as te  # noqa: E402
 import test_emu_hx2 as th  # noqa: E402
+from easu_checks import assert_within_cell_bounds  # noqa: E402
 
 budget = float(sys.argv[1]) if len(sys.argv) > 1 else 300.0
 rng = np.random.default_rng(int(sys.argv[2]) if len(sys.argv) > 2 else 1)
@@ -67,14 +68,23 @@ while time.time() < t_end:
         iw, ih = int(rng.integers(4, 90)), int(rng.integers(4, 40))
         sx, sy = 1.0 + rng.random() * 1.2, 1.0 + rng.random() * 1.2
         ow, oh = max(iw, int(iw * sx)), max(ih, int(ih * sy))
+        # half of the draws render into a viewport of the resource (dynamic resolution), some of those at an offset
+        vw, vh, off = iw, ih, None
+        if rng.integers(2):
+            vw, vh = int(rng.integers(max(1, iw // 2), iw + 1)), int(rng.integers(max(1, ih // 2), ih + 1))
+            ow, oh = max(vw, int(vw * sx)), max(vh, int(vh * sy))
+            if rng.integers(2):
+                off = (int(rng.integers(0, iw - vw + 1)), int(rng.integers(0, ih - vh + 1)))
+        con = ol.easu_con(iw, ih, ow, oh, vw, vh, off=off)
         src = frame(iw, ih)
-        want = ol.easu(src.astype(np.float32), ow, oh)
-        got = te.emu_easu_pairs(src, ow, oh, ctas=int(rng.integers(1, 4)))
+        want = ol.easu(src.astype(np.float32), ow, oh, con)
+        got = te.emu_easu_pairs(src, ow, oh, ctas=int(rng.integers(1, 4)), con=con)
         err = float(np.abs(got.astype(np.float32) - want)[..., :3].max())
-        assert err <= 5e-3, ("easu_any", iw, ih, ow, oh, err)
+        assert err <= 5e-3, ("easu_any", iw, ih, vw, vh, off, ow, oh, err)
+        assert_within_cell_bounds(got, src, con, what=("easu_any", iw, ih, vw, vh, off, ow, oh))
         y0, y1 = rows(oh)
-        part = te.emu_easu_pairs(src, ow, oh, y0=y0, y1=y1, ctas=1)
-        assert np.array_equal(part[y0:y1].view(np.uint16), got[y0:y1].view(np.uint16)), ("easu_any rows", iw, ih, ow, oh, y0, y1)
+        part = te.emu_easu_pairs(src, ow, oh, y0=y0, y1=y1, ctas=1, con=con)
+        assert np.array_equal(part[y0:y1].view(np.uint16), got[y0:y1].view(np.uint16)), ("easu_any rows", iw, ih, vw, vh, off, ow, oh, y0, y1)
         worst["easu_any"] = max(worst["easu_any"], err)
         n["easu_any"] += 1
     elif kind == 2:
