@@ -423,7 +423,9 @@ static int context_run(fsr1_context* c, void* in_dev, uint64_t in_pitch, void* o
   // exactly what FSR_Filter::Upscale passes (sample/src/DX12/FSR_Filter.cpp:106,124)
   fsr1_easu_con(econ, (float)render_w, (float)render_h, (float)render_w, (float)render_h, (float)c->out_w, (float)c->out_h);
   fsr1_rcas_con(rcon, sharpness);
-  return fsr1_upscale(&in, &tmp, &out, econ, rcon, 0, c->out_h, flags, stream);
+  // the context owns the intermediate, so a frame the fused kernel covers takes it; other render sizes, formats and options
+  // fall back to EASU + RCAS through c->tmp
+  return fsr1_upscale(&in, &tmp, &out, econ, rcon, 0, c->out_h, flags | FSR1_FLAG_FUSED, stream);
 }
 
 int fsr1_context_upscale_render(fsr1_context* c, const void* in_dev, uint64_t in_pitch, uint32_t render_w, uint32_t render_h,

@@ -56,12 +56,17 @@ template <int NW> struct __align__(128) FusedSmem {
   uint64_t bar[2];
 };
 
-// EASU output of a quad into the mid tile; pixels outside the image become 0 (what an out-of-image Load returns)
-struct MidSink {
+// EASU output of a quad into the mid tile; pixels outside the image become 0 (what an out-of-image Load returns).
+// kIn: every pixel of the step is inside the image, so nothing is masked.
+template <bool kIn> struct MidSink {
   uint4* top;          // &mid[2r+2][lane]
   bool zT, zB;         // pixel row outside the image
   uint32_t keep;       // per-half mask of the pair: 0xffff low = pixel 2k+1 inside, high = pixel 2k+2 inside
   __device__ __forceinline__ void put(bool bottom, __half2 oR, __half2 oG, __half2 oB) const {
+    if (kIn) {
+      top[bottom ? 32 : 0] = make_uint4(h22u(oR), h22u(oG), h22u(oB), 0u);
+      return;
+    }
     const uint32_t m = (bottom ? zB : zT) ? 0u : keep;
     top[bottom ? 32 : 0] = make_uint4(h22u(oR) & m, h22u(oG) & m, h22u(oB) & m, 0u);
   }
@@ -101,6 +106,64 @@ template <int CY> struct FusedIter {
     return true;
   }
 };
+
+// Phase 3 (EASU of the step's cells into the mid tile), a barrier, then RCAS of the step's output rows.  kIn: an interior step
+// (see the caller): no pixel masked, no row skipped, every store a full pair — a predicate-free copy of the body, as
+// easu_h_quad2x_kernel takes for interior tiles.
+template <bool kIn, int NW>
+__device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams& p, const FusedStep& cur, const uint2* tile, int dx,
+                                           int k0, __half2 sharp, int lane, int warp) {
+  constexpr int CY = FusedCfg<NW>::kCY;
+  const int n = cur.n;
+#pragma unroll 1
+  for (int q = 0; q < 2; q++) {
+    const int r = warp + q * NW;
+    if (!kIn && r >= n) break;  // warp-uniform
+    const int pyT = 2 * (cur.m0 + r) + 1, pxA = 2 * (k0 + lane) + 1;
+    MidSink<kIn> sink;
+    sink.top = &sm.mid[2 * r + 2][lane];
+    sink.zT = !kIn && (pyT < 0 || pyT >= p.out.h);
+    sink.zB = !kIn && (pyT + 1 < 0 || pyT + 1 >= p.out.h);
+    sink.keep = kIn ? 0xffffffffu
+                    : ((pxA >= 0 && pxA < p.out.w) ? 0x0000ffffu : 0u) | ((pxA + 1 >= 0 && pxA + 1 < p.out.w) ? 0xffff0000u : 0u);
+    quad_compute<MidSink<kIn>, kFBW, kFSW>(tile + dx, sm.S + dx, lane, r, true, true, sink);
+  }
+  __syncthreads();
+  // RCAS on the rows whose neighbours are in the mid tile: warp w takes output rows 2 m0 + 4w .. + 3 (mid index 4w+1 ..)
+  constexpr int kR = 2 * CY / NW;  // rows per warp
+  const int o_first = 2 * cur.m0 + warp * kR;
+  const int i0 = warp * kR;        // mid index of the row above the warp's first output row
+  const int lm = lane > 0 ? lane - 1 : 0;
+  const int ox = 2 * (k0 + lane);  // first pixel of the lane's output pair
+  const bool writer = lane >= 1 && (kIn || ox < p.out.w);
+  Row3 E[kR + 2], D[kR], Fv[kR];
+#pragma unroll
+  for (int r = 0; r < kR + 2; r++) {
+    const uint4 a = sm.mid[i0 + r][lm], c = sm.mid[i0 + r][lane];
+    E[r].r = uh2(__byte_perm(a.x, c.x, 0x5432));
+    E[r].g = uh2(__byte_perm(a.y, c.y, 0x5432));
+    E[r].b = uh2(__byte_perm(a.z, c.z, 0x5432));
+    if (r >= 1 && r <= kR) {
+      D[r - 1].r = uh2(a.x); D[r - 1].g = uh2(a.y); D[r - 1].b = uh2(a.z);
+      Fv[r - 1].r = uh2(c.x); Fv[r - 1].g = uh2(c.y); Fv[r - 1].b = uh2(c.z);
+    }
+  }
+  unsigned char* dst = p.out.base + (long long)(o_first - p.out.row0) * p.out.pitch + (long long)ox * 8;
+#pragma unroll
+  for (int r = 0; r < kR; r++) {
+    const int o = o_first + r;
+    if (kIn || (o >= cur.ya && o < cur.yb && o < 2 * cur.m0 + 2 * n)) {  // warp-uniform
+      __half2 oR, oG, oB;
+      rcas_pair<0>(E[r], D[r], E[r + 1], Fv[r], E[r + 2], sharp, oR, oG, oB);
+      if (writer) {
+        const uint4 w = pack_pair_half(oR, oG, oB, 0x3c003c00u);
+        unsigned char* o8 = dst + (long long)r * p.out.pitch;
+        if (kIn || ox + 1 < p.out.w) *reinterpret_cast<uint4*>(o8) = w;
+        else *reinterpret_cast<uint2*>(o8) = make_uint2(w.x, w.y);
+      }
+    }
+  }
+}
 
 template <int NW, int MINB>
 __global__ void __launch_bounds__(NW * 32, MINB)
@@ -153,56 +216,13 @@ fused_h_quad2x_kernel(const FusedParams p, const __grid_constant__ CUtensorMap t
       sm.S[idx] = texel_terms(c[-kFBW], c[-1], c[0], c[1], c[kFBW]);
     }
     __syncthreads();
-    // phase 3: EASU of the step's cells into the mid tile
-#pragma unroll 1
-    for (int q = 0; q < 2; q++) {
-      const int r = warp + q * NW;
-      if (r >= n) break;  // warp-uniform
-      const int pyT = 2 * (cur.m0 + r) + 1, pxA = 2 * (k0 + lane) + 1;
-      MidSink sink;
-      sink.top = &sm.mid[2 * r + 2][lane];
-      sink.zT = pyT < 0 || pyT >= p.out.h;
-      sink.zB = pyT + 1 < 0 || pyT + 1 >= p.out.h;
-      sink.keep = ((pxA >= 0 && pxA < p.out.w) ? 0x0000ffffu : 0u) | ((pxA + 1 >= 0 && pxA + 1 < p.out.w) ? 0xffff0000u : 0u);
-      quad_compute<MidSink, kFBW, kFSW>(tile + dx, sm.S + dx, lane, r, true, true, sink);
-    }
-    __syncthreads();
-    // RCAS on the rows whose neighbours are in the mid tile: warp w takes output rows 2 m0 + 4w .. + 3 (mid index 4w+1 ..)
-    {
-      constexpr int kR = 2 * CY / NW;  // rows per warp
-      const int o_first = 2 * cur.m0 + warp * kR;
-      const int i0 = warp * kR;        // mid index of the row above the warp's first output row
-      const int lm = lane > 0 ? lane - 1 : 0;
-      const int ox = 2 * (k0 + lane);  // first pixel of the lane's output pair
-      const bool writer = lane >= 1 && ox < p.out.w;
-      Row3 E[kR + 2], D[kR], Fv[kR];
-#pragma unroll
-      for (int r = 0; r < kR + 2; r++) {
-        const uint4 a = sm.mid[i0 + r][lm], c = sm.mid[i0 + r][lane];
-        E[r].r = uh2(__byte_perm(a.x, c.x, 0x5432));
-        E[r].g = uh2(__byte_perm(a.y, c.y, 0x5432));
-        E[r].b = uh2(__byte_perm(a.z, c.z, 0x5432));
-        if (r >= 1 && r <= kR) {
-          D[r - 1].r = uh2(a.x); D[r - 1].g = uh2(a.y); D[r - 1].b = uh2(a.z);
-          Fv[r - 1].r = uh2(c.x); Fv[r - 1].g = uh2(c.y); Fv[r - 1].b = uh2(c.z);
-        }
-      }
-      unsigned char* dst = p.out.base + (long long)(o_first - p.out.row0) * p.out.pitch + (long long)ox * 8;
-#pragma unroll
-      for (int r = 0; r < kR; r++) {
-        const int o = o_first + r;
-        if (o >= cur.ya && o < cur.yb && o < 2 * cur.m0 + 2 * n) {  // warp-uniform
-          __half2 oR, oG, oB;
-          rcas_pair<0>(E[r], D[r], E[r + 1], Fv[r], E[r + 2], sharp, oR, oG, oB);
-          if (writer) {
-            const uint4 w = pack_pair_half(oR, oG, oB, 0x3c003c00u);
-            unsigned char* o8 = dst + (long long)r * p.out.pitch;
-            if (ox + 1 < p.out.w) *reinterpret_cast<uint4*>(o8) = w;
-            else *reinterpret_cast<uint2*>(o8) = make_uint2(w.x, w.y);
-          }
-        }
-      }
-    }
+    // interior step: the strip's cells and pixels are in the image (k0 >= 0, m0 >= 0, last pixel column and row inside), the step
+    // is full (n = CY) and every output row it produces lies in [ya, yb) — never the first step of a run, whose first two output
+    // rows lie above ya
+    const bool inside = k0 >= 0 && 2 * (k0 + 31) + 2 < p.out.w && cur.m0 >= 0 && 2 * (cur.m0 + CY) < p.out.h && n == CY &&
+                        2 * cur.m0 >= cur.ya && 2 * (cur.m0 + CY) <= cur.yb;
+    if (inside) fused_step<true>(sm, p, cur, tile, dx, k0, sharp, lane, warp);
+    else fused_step<false>(sm, p, cur, tile, dx, k0, sharp, lane, warp);
     __syncthreads();
     if (n == CY && tid < 64) {  // the run may continue: its last two mid rows become rows 0, 1 of the next step
       const int rr = tid >> 5;
@@ -239,12 +259,14 @@ cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cu
   // output pairs (2k, 2k+1), k = 0 .. (w-1)/2, 31 per strip
   p.n_strips = ((e.out.w + 1) / 2 + kStripCells - 1) / kStripCells;
   const long long units = (long long)p.n_strips * ((e.y1 - e.y0 + 1) / 2);
-  constexpr int kPerSM = 6;
-  long long grid = (long long)kPerSM * sm_count();
+  // 72 registers = 7 CTAs per SM, as easu_h_quad2x; a launch that waits for a neighbour's halo (p.sync) takes 6 so that the
+  // one-warp halo_push_kernel it waits for still fits beside it (launch_easu_h_tiled, DESIGN.md §6)
+  const int per_sm = (p.sync.ready[0] || p.sync.ready[1]) ? 6 : 7;
+  long long grid = (long long)per_sm * sm_count();
   if (grid > (units + 7) / 8) grid = (units + 7) / 8;  // at least ~16 rows of a strip per CTA
   if (grid < 1) grid = 1;
-  fused_h_quad2x_kernel<NW, kPerSM><<<(int)grid, NW * 32, 0, s>>>(p, tmap);
-  *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips>";
+  fused_h_quad2x_kernel<NW, 7><<<(int)grid, NW * 32, 0, s>>>(p, tmap);
+  *name = per_sm == 7 ? "fused_easu_rcas_h_quad2x<4w,7/sm,tma2,strips>" : "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips>";
   return cudaGetLastError();
 }
 #endif

@@ -130,7 +130,7 @@ struct fsr1_shard {
   bool peer_is_ipc[2];
   uint32_t peer_win0[2];       // first logical row of the neighbour's window
   Rows send[2];                // my rows the neighbour needs
-  unsigned char* tmp;          // slots x rows easu_rows
+  unsigned char* tmp;          // slots x rows easu_rows; null when the frames take the fused kernel (no intermediate)
   unsigned char* out;          // slots x rows out_rows
   uint64_t out_pitch, tmp_slot_stride, out_slot_stride;
   uint32_t seq[kMaxSlots];
@@ -229,7 +229,6 @@ int fsr1_shard_create(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);  // numerically lowest = most urgent
   // cudaMalloc (not a pool / VMM allocation): the arena must be exportable through cudaIpcGetMemHandle
   if ((e = cudaMalloc((void**)&s->arena, s->arena_bytes)) != cudaSuccess || (e = cudaMemset(s->arena, 0, s->arena_bytes)) != cudaSuccess ||
-      (e = cudaMalloc((void**)&s->tmp, s->tmp_slot_stride * slots)) != cudaSuccess ||
       (e = cudaMalloc((void**)&s->out, s->out_slot_stride * slots)) != cudaSuccess ||
       (e = cudaStreamCreateWithPriority(&s->s_comm, cudaStreamNonBlocking, prio_hi)) != cudaSuccess ||
       (e = cudaStreamCreateWithFlags(&s->s_easu, cudaStreamNonBlocking)) != cudaSuccess ||
@@ -251,27 +250,42 @@ int fsr1_shard_create(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_
     }
   }
   if (world > 1) {
-    // Load every kernel a frame uses NOW.  CUDA loads kernels lazily, on first launch, and loading may synchronise the context: a
-    // first-use load issued while a flag-waiting kernel spins would wait for that kernel, which (several ranks in ONE process) may be
-    // waiting for work this very host thread has not submitted yet.  One dry frame on the zero-filled slot 0 (no halo protocol).
     cudaFuncAttributes fa;
     if (cudaFuncGetAttributes(&fa, halo_push_kernel) != cudaSuccess || cudaFuncGetAttributes(&fa, halo_wait_kernel) != cudaSuccess ||
         cudaFuncGetAttributes(&fa, credit_signal_kernel) != cudaSuccess) {
       fsr1_shard_destroy(s);
       return FSR1_ERR_CUDA;
     }
+  }
+  // One dry frame on the zero-filled slot 0 (no halo protocol).  Every frame of the shard has this frame's format, scale, layout and
+  // options, so it decides for all of them:
+  //  - whether they take the fused EASU->RCAS kernel.  It is tried first, without an intermediate; only a configuration it does not
+  //    cover (fsr1_upscale then needs `tmp`) gets the intermediate, 66 MB per slot at 1080p->4K RGBA16F, and runs the frame again
+  //    through the two kernels;
+  //  - whether the kernel takes the halo hand-shake itself (null pointers: a no-op inside the kernel);
+  //  - and it loads every kernel a frame uses NOW.  CUDA loads kernels lazily, on first launch, and loading may synchronise the
+  //    context: a first-use load issued while a flag-waiting kernel spins would wait for that kernel, which (several ranks in ONE
+  //    process) may be waiting for work this very host thread has not submitted yet.
+  {
     fsr1_image win, out;
     fsr1_shard_window(s, 0, &win);
     fsr1_shard_output(s, 0, &out);
-    fsr1_image tmp0 = {s->tmp, s->out_pitch, s->out_w, s->out_h, s->easu_rows.a, s->easu_rows.b - s->easu_rows.a, s->format, 0};
-    const uint32_t kflags = flags & ~(uint32_t)(FSR1_SHARD_ONE_STREAM | FSR1_SHARD_SKIP_HALO | FSR1_SHARD_TRACE);
+    const uint32_t kflags = (flags & ~(uint32_t)(FSR1_SHARD_ONE_STREAM | FSR1_SHARD_SKIP_HALO | FSR1_SHARD_TRACE)) | FSR1_FLAG_FUSED;
     const fsr1::HaloSync none = {};
-    fsr1::set_halo_sync(&none);  // does this configuration's kernel take the hand-shake? (null pointers: a no-op inside the kernel)
-    int rc = fsr1_upscale(&win, &tmp0, &out, s->econ, s->rcon, s->out_rows.a, s->out_rows.b, kflags, s->s_easu);
+    fsr1::set_halo_sync(&none);
+    int rc = fsr1_upscale(&win, nullptr, &out, s->econ, s->rcon, s->out_rows.a, s->out_rows.b, kflags, s->s_easu);
+    if (rc != FSR1_OK) {
+      if ((e = cudaMalloc((void**)&s->tmp, s->tmp_slot_stride * slots)) != cudaSuccess) {
+        fsr1::set_halo_sync(nullptr);
+        fsr1_shard_destroy(s);
+        return FSR1_ERR_CUDA;
+      }
+      fsr1_image tmp0 = {s->tmp, s->out_pitch, s->out_w, s->out_h, s->easu_rows.a, s->easu_rows.b - s->easu_rows.a, s->format, 0};
+      fsr1::set_halo_sync(&none);
+      rc = fsr1_upscale(&win, &tmp0, &out, s->econ, s->rcon, s->out_rows.a, s->out_rows.b, kflags, s->s_easu);
+    }
     s->inkernel_sync = fsr1::halo_sync_consumed();
     fsr1::set_halo_sync(nullptr);
-    if (rc == FSR1_OK && (kflags & FSR1_FLAG_FUSED))  // the fused path may fall back to the two kernels for other frames: load those too
-      rc = fsr1_upscale(&win, &tmp0, &out, s->econ, s->rcon, s->out_rows.a, s->out_rows.b, kflags & ~(uint32_t)FSR1_FLAG_FUSED, s->s_easu);
     if (rc != FSR1_OK) { fsr1_shard_destroy(s); return rc; }
   }
   if ((e = cudaDeviceSynchronize()) != cudaSuccess) { fsr1_shard_destroy(s); return FSR1_ERR_CUDA; }  // flags are zero before anyone attaches
@@ -438,13 +452,15 @@ int fsr1_shard_submit(fsr1_shard* s, uint32_t slot, void* stream) {
   fsr1_image win, out;
   fsr1_shard_window(s, slot, &win);
   fsr1_shard_output(s, slot, &out);
-  fsr1_image tmp = make_img(s->tmp + (uint64_t)slot * s->tmp_slot_stride, s->out_pitch, s->out_w, s->out_h, s->easu_rows.a,
-                            s->easu_rows.b - s->easu_rows.a, s->format);
-  const uint32_t kflags = s->flags & ~(uint32_t)(FSR1_SHARD_ONE_STREAM | FSR1_SHARD_SKIP_HALO | FSR1_SHARD_TRACE);
-  const bool fused = (kflags & FSR1_FLAG_FUSED) != 0;
-  // The whole frame runs on ONE stream, consecutive frames on the two streams in turn: RCAS of frame i (ALU / XU / HBM-bound) overlaps
-  // EASU of frame i+1 (FMA-pipe-bound) without an event between the two kernels of a frame, three driver calls fewer per frame than
-  // "EASU of every frame on one stream, RCAS on the other".
+  fsr1_image tmp;
+  if (s->tmp)
+    tmp = make_img(s->tmp + (uint64_t)slot * s->tmp_slot_stride, s->out_pitch, s->out_w, s->out_h, s->easu_rows.a,
+                   s->easu_rows.b - s->easu_rows.a, s->format);
+  // fused whenever the kernel covers the frame (fsr1_shard_create allocated no intermediate then), else EASU + RCAS through `tmp`
+  const uint32_t kflags = (s->flags & ~(uint32_t)(FSR1_SHARD_ONE_STREAM | FSR1_SHARD_SKIP_HALO | FSR1_SHARD_TRACE)) | FSR1_FLAG_FUSED;
+  // The whole frame runs on ONE stream, consecutive frames on the two streams in turn: the tail of frame i overlaps the start of
+  // frame i+1 (and with two kernels, RCAS of frame i (ALU / XU / HBM-bound) overlaps EASU of frame i+1 (FMA-pipe-bound)) without an
+  // event between the kernels of a frame.
   cudaStream_t sk = (!one_stream && (s->frames & 1)) ? sr : se;
   if ((e = cudaStreamWaitEvent(sk, s->ev_in[slot], 0)) != cudaSuccess) return cuda_rc(e);
   if (q > 1 && !one_stream && (e = cudaStreamWaitEvent(sk, s->ev_rcas[slot], 0)) != cudaSuccess) return cuda_rc(e);  // the slot's intermediate / output are free
@@ -463,8 +479,7 @@ int fsr1_shard_submit(fsr1_shard* s, uint32_t slot, void* stream) {
     if ((e = cudaGetLastError()) != cudaSuccess) return cuda_rc(e);
   }
   if (inkernel) fsr1::set_halo_sync(&hs);
-  int rc = fused ? fsr1_upscale(&win, &tmp, &out, s->econ, s->rcon, s->out_rows.a, s->out_rows.b, kflags, sk)
-                 : fsr1_easu(&win, &tmp, s->econ, s->easu_rows.a, s->easu_rows.b, kflags & ~(uint32_t)FSR1_FLAG_OUTPUT_SQUARE, sk);
+  int rc = fsr1_upscale(&win, s->tmp ? &tmp : nullptr, &out, s->econ, s->rcon, s->out_rows.a, s->out_rows.b, kflags, sk);
   const bool took = inkernel && fsr1::halo_sync_consumed();
   fsr1::set_halo_sync(nullptr);
   if (rc != FSR1_OK) return rc;
@@ -472,10 +487,6 @@ int fsr1_shard_submit(fsr1_shard* s, uint32_t slot, void* stream) {
   if (shake && !inkernel) {
     credit_signal_kernel<<<1, 32, 0, sk>>>(hs.credit[kFromUp], hs.credit[kFromDown], q);
     if ((e = cudaGetLastError()) != cudaSuccess) return cuda_rc(e);
-  }
-  if (!fused) {
-    rc = fsr1_rcas(&tmp, &out, s->rcon, s->out_rows.a, s->out_rows.b, kflags, sk);
-    if (rc != FSR1_OK) return rc;
   }
   if ((e = cudaEventRecord(s->ev_rcas[slot], sk)) != cudaSuccess) return cuda_rc(e);
   return FSR1_OK;

@@ -77,7 +77,9 @@ enum {
   FSR1_FLAG_FUSED = 1u << 9,        /* fsr1_upscale*: EASU and RCAS in ONE kernel where one exists (RGBA16F, exactly 2x, out-of-image
                                        RCAS taps read 0, no RCAS options): the intermediate stays in shared memory, `tmp` is not
                                        touched, HBM traffic drops from 26 to 10 bytes per output pixel; results are bit-identical
-                                       to the two-kernel path.  Falls back to the two kernels otherwise. */
+                                       to the two-kernel path.  Falls back to the two kernels otherwise.  fsr1_shard_* and
+                                       fsr1_context_* own their intermediate and take the fused kernel automatically; the flag
+                                       only matters for fsr1_upscale, whose caller passes `tmp`. */
   FSR1_FLAG_RCAS_HX2 = 1u << 10,    /* fsr1_rcas, fp16 images only: the reference's PACKED calling convention FsrRcasHx2 +
                                        FsrRcasDepackHx2 (ffx_fsr1.h:880-984): each lane sharpens pixels ip and ip + (8,0) held as
                                        half2 structure-of-arrays registers, every operation a packed half operation with its own
@@ -149,12 +151,13 @@ int fsr1_context_upscale_host(fsr1_context* ctx, const void* in_host, uint64_t i
  * The output image is cut into `world` contiguous row slabs, one per rank (= per GPU).  Rank k owns input rows
  * [k*in_h/world, (k+1)*in_h/world) and needs 2-3 more rows each side: the EASU footprint of its slab plus the
  * one-row apron RCAS reads, so there is exactly ONE neighbour exchange per frame and no collective.
- * A fsr1_shard owns the rank's share of a ring of `slots` frames: input window (own rows + halo), intermediate,
- * output slab, three internal streams.  The halo moves by direct NVLink stores into the neighbour's window
+ * A fsr1_shard owns the rank's share of a ring of `slots` frames: input window (own rows + halo), output slab,
+ * three internal streams, and an intermediate only when its frames cannot take the fused EASU->RCAS kernel (see
+ * FSR1_FLAG_FUSED; decided at create time).  The halo moves by direct NVLink stores into the neighbour's window
  * (CUDA IPC between processes, peer access inside one process), flow-controlled by sequence numbers in device
  * memory: no NCCL call, no host synchronisation and no allocation per frame.  Per frame the caller writes its
  * input rows into fsr1_shard_input(slot) on `stream`, calls fsr1_shard_submit(slot, stream), and orders its
- * consumer after fsr1_shard_wait(slot, stream).  RCAS of frame i overlaps EASU of frame i+1 on every rank.
+ * consumer after fsr1_shard_wait(slot, stream).  Consecutive frames run on two streams in turn and overlap.
  * All ranks must create shards with identical arguments (except rank) and submit slots in the same order.
  * Set-up between processes: every rank calls fsr1_shard_export, the 64-byte handles are gathered in rank order by
  * any means (torch.distributed all_gather, MPI, a pipe), every rank calls fsr1_shard_attach.  In one process
