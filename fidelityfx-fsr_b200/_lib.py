@@ -10,11 +10,12 @@ FSR1_OK = 0
 FORMAT_RGBA16F, FORMAT_RGBA32F, FORMAT_RGBA8_UNORM, FORMAT_RGB10A2_UNORM = 1, 2, 3, 4
 FLAG_RCAS_CLAMP, FLAG_EXACT, FLAG_FORCE_DIRECT, FLAG_NO_RCAS, FLAG_H_REFERENCE, FLAG_PRECISE = 1, 2, 4, 8, 16, 32
 FLAG_RCAS_DENOISE, FLAG_RCAS_PASSTHROUGH_ALPHA, FLAG_OUTPUT_SQUARE, FLAG_FUSED, FLAG_RCAS_HX2 = 64, 128, 256, 512, 1024
+POST_SRTM_INVERSE, POST_LFGA, POST_TEPD8, POST_TEPD10 = 1, 2, 4, 8
 SHARD_ONE_STREAM, SHARD_SKIP_HALO, SHARD_TRACE, SHARD_HANDLE_BYTES = 1 << 16, 1 << 17, 1 << 18, 64
 
 # every symbol include/fsr1_b200.h declares
-SYMBOLS = ["fsr1_easu", "fsr1_rcas", "fsr1_easu_input_rows", "fsr1_upscale", "fsr1_context_create",
-           "fsr1_context_destroy", "fsr1_context_upscale", "fsr1_context_upscale_render", "fsr1_context_upscale_host", "fsr1_easu_con",
+SYMBOLS = ["fsr1_easu", "fsr1_rcas", "fsr1_easu_input_rows", "fsr1_upscale", "fsr1_upscale_post", "fsr1_context_create",
+           "fsr1_context_destroy", "fsr1_context_upscale", "fsr1_context_upscale_render", "fsr1_context_upscale_post", "fsr1_context_upscale_host", "fsr1_easu_con",
            "fsr1_easu_con_offset", "fsr1_rcas_con", "fsr1_abi_version", "fsr1_error_string",
            "fsr1_last_cuda_error", "fsr1_launch_count", "fsr1_last_kernel_name", "fsr1_srtm", "fsr1_lfga", "fsr1_tepd",
            "fsr1_srtm_h", "fsr1_lfga_h", "fsr1_tepd_h",
@@ -28,6 +29,12 @@ class Image(ctypes.Structure):
     _fields_ = [("data", ctypes.c_void_p), ("pitch_bytes", ctypes.c_uint64), ("width", ctypes.c_uint32),
                 ("height", ctypes.c_uint32), ("row0", ctypes.c_uint32), ("rows", ctypes.c_uint32),
                 ("format", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class Post(ctypes.Structure):
+    """struct fsr1_post"""
+    _fields_ = [("ops", ctypes.c_uint32), ("lfga_amount", ctypes.c_float), ("grain", ctypes.POINTER(Image)),
+                ("dither", ctypes.POINTER(Image)), ("frame", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
 
 
 class ShardInfo(ctypes.Structure):
@@ -59,6 +66,9 @@ def lib():
     L.fsr1_rcas.argtypes = [imgp, imgp, u32p, u32, u32, u32, vp]
     L.fsr1_easu_input_rows.argtypes = [u32p, u32, u32, u32, u32p, u32p]
     L.fsr1_upscale.argtypes = [imgp, imgp, imgp, u32p, u32p, u32, u32, u32, vp]
+    postp = ctypes.POINTER(Post)
+    L.fsr1_upscale_post.argtypes = [imgp, imgp, imgp, u32p, u32p, postp, u32, u32, u32, vp]
+    L.fsr1_context_upscale_post.argtypes = [vp, vp, u64, u32, u32, vp, u64, f32, postp, u32, vp]
     L.fsr1_context_create.argtypes = [ctypes.POINTER(vp), u32, u32, u32, u32, u32]
     L.fsr1_context_destroy.argtypes = [vp]
     L.fsr1_context_destroy.restype = None

@@ -10,6 +10,7 @@ import torch
 from . import _lib
 from ._lib import FORMAT_RGB10A2_UNORM, FORMAT_RGBA8_UNORM  # noqa: F401
 from ._lib import FLAG_FUSED, FLAG_OUTPUT_SQUARE, FLAG_RCAS_HX2  # noqa: F401
+from ._lib import POST_LFGA, POST_SRTM_INVERSE, POST_TEPD10, POST_TEPD8  # noqa: F401
 from ._lib import (FLAG_EXACT, FLAG_FORCE_DIRECT, FLAG_H_REFERENCE, FLAG_NO_RCAS, FLAG_PRECISE, FLAG_RCAS_DENOISE, FLAG_RCAS_PASSTHROUGH_ALPHA, FLAG_RCAS_CLAMP, FORMAT_RGBA16F,  # noqa: F401
                    FORMAT_RGBA32F, Fsr1Error, Image)
 
@@ -95,6 +96,33 @@ def upscale(inp, tmp, out, econ, rcon, y0=0, y1=0, flags=0, stream=None):
     a, t, b = _as_img(inp), _as_img(tmp), _as_img(out)
     _lib.check(_lib.lib().fsr1_upscale(ctypes.byref(a), ctypes.byref(t), ctypes.byref(b), (ctypes.c_uint32 * 16)(*econ),
                                        (ctypes.c_uint32 * 4)(*rcon), y0, y1, flags, _stream(stream)))
+
+
+def _post(srtm_inverse, grain, amount, tepd_bits, dither, frame):
+    """struct fsr1_post for the given steps, and the image descriptors it points at (kept alive by the caller)."""
+    if tepd_bits not in (0, 8, 10):
+        raise Fsr1Error("tepd_bits must be 0, 8 or 10")
+    ops = (_lib.POST_SRTM_INVERSE if srtm_inverse else 0) | (_lib.POST_LFGA if grain is not None else 0)
+    ops |= {0: 0, 8: _lib.POST_TEPD8, 10: _lib.POST_TEPD10}[tepd_bits]
+    g = _as_img(grain) if grain is not None else None
+    d = _as_img(dither) if dither is not None and tepd_bits else None
+    post = _lib.Post(ops, amount, ctypes.pointer(g) if g is not None else None, ctypes.pointer(d) if d is not None else None, frame, 0)
+    return post, (g, d)
+
+
+def upscale_post(inp, tmp, out, econ, rcon, srtm_inverse=False, grain=None, amount=0.0, tepd_bits=0, dither=None, frame=0, y0=0, y1=0,
+                 flags=0, stream=None):
+    """upscale() followed by SRTM inverse, LFGA (when `grain` is given) and TEPD (tepd_bits 8 / 10), applied inside RCAS's store:
+    the bits of upscale + srtm(inverse) + lfga + tepd through an RGBA16F intermediate, written once.  `out` is float16 [H,W,4], or with
+    TEPD uint8 [H,W,4] (8 bits) / int32 [H,W] (10 bits), as tepd() accepts.  `tmp` may be None when the frame takes the fused kernel
+    (FLAG_FUSED, exactly 2x, no RCAS option)."""
+    a, b = _as_img(inp), _as_img(out)
+    t = _as_img(tmp) if tmp is not None else None
+    post, keep = _post(srtm_inverse, grain, amount, tepd_bits, dither, frame)
+    _lib.check(_lib.lib().fsr1_upscale_post(ctypes.byref(a), ctypes.byref(t) if t is not None else None, ctypes.byref(b),
+                                            (ctypes.c_uint32 * 16)(*econ), (ctypes.c_uint32 * 4)(*rcon), ctypes.byref(post), y0, y1,
+                                            flags, _stream(stream)))
+    del keep
 
 
 def srtm(inp, out, inverse=False, y0=0, y1=0, stream=None):
@@ -252,6 +280,17 @@ class HostContext:
             self._h, ctypes.c_void_p(in_dev.data_ptr()), in_dev.stride(0) * in_dev.element_size(), render_w, render_h,
             ctypes.c_void_p(out_dev.data_ptr()), out_dev.stride(0) * out_dev.element_size(),
             ctypes.c_float(sharpness), flags, _stream(stream)))
+
+    def upscale_post(self, in_dev, out_dev, render_w=0, render_h=0, sharpness=0.25, srtm_inverse=False, grain=None, amount=0.0,
+                     tepd_bits=0, dither=None, frame=0, flags=0, stream=None):
+        """fsr1_context_upscale_post: upscale_render followed by the display steps of api.upscale_post; `out_dev` is uint8 [H,W,4]
+        with tepd_bits 8, int32 [H,W] with 10, float16 [H,W,4] otherwise.  render size 0 = the context's input size."""
+        post, keep = _post(srtm_inverse, grain, amount, tepd_bits, dither, frame)
+        _lib.check(_lib.lib().fsr1_context_upscale_post(
+            self._h, ctypes.c_void_p(in_dev.data_ptr()), in_dev.stride(0) * in_dev.element_size(), render_w, render_h,
+            ctypes.c_void_p(out_dev.data_ptr()), out_dev.stride(0) * out_dev.element_size(), ctypes.c_float(sharpness),
+            ctypes.byref(post), flags, _stream(stream)))
+        del keep
 
     def close(self):
         if self._h:

@@ -11,6 +11,7 @@
 #include "../../include/fsr1_b200.h"
 #include "../../include/fsr1_host.h"
 #include "fsr1_common.cuh"
+#include "fsr1_post.cuh"
 
 using namespace fsr1;
 
@@ -343,6 +344,109 @@ int fsr1_upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
   return fsr1_rcas(tmp, out, rcas_con, y0, y1, flags, stream);
 }
 
+// ---- upscale straight to the display output ----------------------------------------------------------------
+namespace {
+constexpr uint32_t kAllPost = FSR1_POST_SRTM_INVERSE | FSR1_POST_LFGA | FSR1_POST_TEPD8 | FSR1_POST_TEPD10;
+
+// an aux tile of the epilogue: a whole image (not a window), described as 1 x 1 when the ops do not read it
+int post_tile(const fsr1_image* im, bool used, ImgView& v, int& fmt) {
+  v = ImgView{nullptr, 0, 1, 1, 0, 1};
+  fmt = 0;
+  if (!used || !im) return FSR1_OK;
+  const int rc = check_image(im);
+  if (rc != FSR1_OK) return rc;
+  if (im->row0 != 0 || im->rows != im->height) return FSR1_ERR_INVALID_ARGUMENT;
+  v = view_of(im);
+  fmt = (int)im->format;
+  return FSR1_OK;
+}
+}  // namespace
+
+int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, const uint32_t easu_con[16],
+                      const uint32_t rcas_con[4], const fsr1_post* post, uint32_t y0, uint32_t y1, uint32_t flags, void* stream) {
+  if (!post || post->ops == 0) return fsr1_upscale(in, tmp, out, easu_con, rcas_con, y0, y1, flags, stream);
+  NvtxRange range("FSR1 upscale post");
+  const uint32_t ops = post->ops;
+  if (ops & ~kAllPost) return FSR1_ERR_INVALID_ARGUMENT;
+  if ((ops & FSR1_POST_TEPD8) && (ops & FSR1_POST_TEPD10)) return FSR1_ERR_INVALID_ARGUMENT;
+  if ((ops & FSR1_POST_LFGA) && !post->grain) return FSR1_ERR_INVALID_ARGUMENT;
+  int rc;
+  if ((rc = check_image(in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
+  if (!easu_con || !rcas_con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
+  PostParams q;
+  const bool tepd = (ops & (FSR1_POST_TEPD8 | FSR1_POST_TEPD10)) != 0;
+  if ((rc = post_tile(post->grain, (ops & FSR1_POST_LFGA) != 0, q.grain, q.grain_fmt)) != FSR1_OK) return rc;
+  if ((rc = post_tile(post->dither, tepd, q.dither, q.dither_fmt)) != FSR1_OK) return rc;
+  if (q.grain_fmt && q.grain_fmt != FSR1_FORMAT_RGBA16F && q.grain_fmt != FSR1_FORMAT_RGBA32F) return FSR1_ERR_UNSUPPORTED;  // signed values
+  q.ops = (int)ops;
+  q.amount = post->lfga_amount;
+  q.frame = post->frame;
+  // formats: RGBA16F in; RGBA16F out, or with TEPD the matching UNORM code values (the rule of fsr1_tepd)
+  if (in->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
+  const uint32_t unorm = (ops & FSR1_POST_TEPD8) ? FSR1_FORMAT_RGBA8_UNORM : (ops & FSR1_POST_TEPD10) ? FSR1_FORMAT_RGB10A2_UNORM : 0;
+  if (out->format != FSR1_FORMAT_RGBA16F && (!unorm || out->format != unorm)) return FSR1_ERR_UNSUPPORTED;
+  // the half-arithmetic parity paths, fp32 EXACT/direct kernels and EASU-only frames keep the separate passes
+  if (flags & (FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_RCAS_HX2 | FSR1_FLAG_NO_RCAS))
+    return FSR1_ERR_UNSUPPORTED;
+  if (y1 == 0) y1 = out->height;
+  if (y0 >= y1 || y1 > out->height) return FSR1_ERR_INVALID_ARGUMENT;
+  if (!window_holds(out, (int)y0, (int)y1 - 1)) return FSR1_ERR_WINDOW;
+  const uint32_t e0 = y0 == 0 ? 0 : y0 - 1, e1 = y1 >= out->height ? out->height : y1 + 1;  // EASU rows incl. RCAS's apron
+  uint32_t r0, r1;
+  fsr1_easu_input_rows(easu_con, in->height, e0, e1, &r0, &r1);
+  if (!window_holds(in, (int)r0, (int)r1)) return FSR1_ERR_WINDOW;
+  const int out_align = out->format == FSR1_FORMAT_RGBA16F ? 16 : 8;
+  if (((uintptr_t)out->data & (out_align - 1)) || (out->pitch_bytes & (out_align - 1))) return FSR1_ERR_UNSUPPORTED;
+  if (tmp) {  // the intermediate of the two-kernel path (unused by the fused kernel)
+    if ((rc = check_image(tmp)) != FSR1_OK) return rc;
+    if (tmp->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
+    if (tmp->width != out->width || tmp->height != out->height) return FSR1_ERR_INVALID_ARGUMENT;
+    if (!window_holds(tmp, (int)e0, (int)e1 - 1)) return FSR1_ERR_WINDOW;
+    if (((uintptr_t)tmp->data & 15) || (tmp->pitch_bytes & 15)) return FSR1_ERR_UNSUPPORTED;
+    {  // RCAS reads neighbours of every pixel it writes
+      const uintptr_t a0 = (uintptr_t)tmp->data, a1 = a0 + (uintptr_t)tmp->pitch_bytes * tmp->rows;
+      const uintptr_t b0 = (uintptr_t)out->data, b1 = b0 + (uintptr_t)out->pitch_bytes * out->rows;
+      if (a0 < b1 && b0 < a1) return FSR1_ERR_INVALID_ARGUMENT;
+    }
+  }
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const char* name = "";
+
+  EasuParams e;
+  e.in = view_of(in);
+  e.out = view_of(out);
+  e.c0x = as_float(easu_con[0]); e.c0y = as_float(easu_con[1]); e.c0z = as_float(easu_con[2]); e.c0w = as_float(easu_con[3]);
+  e.y0 = (int)y0; e.y1 = (int)y1;
+  if ((flags & FSR1_FLAG_FUSED) && !(flags & (FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_CLAMP | FSR1_FLAG_RCAS_DENOISE |
+                                              FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA | FSR1_FLAG_OUTPUT_SQUARE))) {
+    const cudaError_t err = launch_fused_h_post(e, rcas_con[1], q, (int)out->format, s, &name);
+    if (err == cudaSuccess) {
+      t_last_kernel = name;
+      g_launches.fetch_add(1);
+      return FSR1_OK;
+    }
+    if (err != cudaErrorNotSupported) return cuda_fail(err);
+  }
+  // EASU into tmp (as fsr1_upscale does), then RCAS with the epilogue in its store
+  if (!tmp) return FSR1_ERR_INVALID_ARGUMENT;
+  rc = fsr1_easu(in, tmp, easu_con, e0, e1, flags & ~(uint32_t)(FSR1_FLAG_FUSED | FSR1_FLAG_OUTPUT_SQUARE), stream);
+  if (rc != FSR1_OK) return rc;
+  RcasParams p;
+  p.in = view_of(tmp);
+  p.out = view_of(out);
+  p.sharp = as_float(rcas_con[0]);
+  p.sharp_h2 = rcas_con[1];
+  p.y0 = (int)y0; p.y1 = (int)y1;
+  p.clamp = (flags & FSR1_FLAG_RCAS_CLAMP) ? 1 : 0;
+  p.options = ((flags & FSR1_FLAG_RCAS_DENOISE) ? 1 : 0) | ((flags & FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA) ? 2 : 0) |
+              ((flags & FSR1_FLAG_OUTPUT_SQUARE) ? 4 : 0);
+  const cudaError_t err = launch_rcas_h_post(p, q, (int)out->format, s, &name);
+  if (err != cudaSuccess) return err == cudaErrorNotSupported ? FSR1_ERR_UNSUPPORTED : cuda_fail(err);
+  t_last_kernel = name;
+  g_launches.fetch_add(1);
+  return FSR1_OK;
+}
+
 // ---- pointwise companions ------------------------------------------------------------------------------
 int fsr1_srtm(const fsr1_image* in, const fsr1_image* out, int inverse, uint32_t y0, uint32_t y1, void* stream) {
   return pointwise(inverse ? 2 : 1, in, nullptr, out, 0.0f, 0u, y0, y1, stream);
@@ -433,6 +537,27 @@ int fsr1_context_upscale_render(fsr1_context* c, const void* in_dev, uint64_t in
   if (!c || !in_dev || !out_dev || !render_w || !render_h) return FSR1_ERR_INVALID_ARGUMENT;
   if (render_w > c->in_w || render_h > c->in_h) return FSR1_ERR_INVALID_ARGUMENT;  // would read past the caller's input
   return context_run(c, const_cast<void*>(in_dev), in_pitch, out_dev, out_pitch, sharpness, flags, stream, render_w, render_h);
+}
+
+int fsr1_context_upscale_post(fsr1_context* c, const void* in_dev, uint64_t in_pitch, uint32_t render_w, uint32_t render_h,
+                              void* out_dev, uint64_t out_pitch, float sharpness, const fsr1_post* post, uint32_t flags, void* stream) {
+  if (!c || !in_dev || !out_dev) return FSR1_ERR_INVALID_ARGUMENT;
+  if (c->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
+  if (render_w == 0) render_w = c->in_w;
+  if (render_h == 0) render_h = c->in_h;
+  if (render_w > c->in_w || render_h > c->in_h) return FSR1_ERR_INVALID_ARGUMENT;  // would read past the caller's input
+  // the output's format follows the ops: with TEPD the matching UNORM code values (the display image), otherwise RGBA16F
+  const uint32_t ops = post ? post->ops : 0u;
+  uint32_t ofmt = FSR1_FORMAT_RGBA16F;
+  if ((ops & FSR1_POST_TEPD10) && !(ops & FSR1_POST_TEPD8)) ofmt = FSR1_FORMAT_RGB10A2_UNORM;
+  if ((ops & FSR1_POST_TEPD8) && !(ops & FSR1_POST_TEPD10)) ofmt = FSR1_FORMAT_RGBA8_UNORM;
+  fsr1_image in = {const_cast<void*>(in_dev), in_pitch, render_w, render_h, 0, render_h, c->format, 0};
+  fsr1_image tmp = {c->tmp, c->tmp_pitch, c->out_w, c->out_h, 0, c->out_h, c->format, 0};
+  fsr1_image out = {out_dev, out_pitch, c->out_w, c->out_h, 0, c->out_h, ofmt, 0};
+  uint32_t econ[16], rcon[4];
+  fsr1_easu_con(econ, (float)render_w, (float)render_h, (float)render_w, (float)render_h, (float)c->out_w, (float)c->out_h);
+  fsr1_rcas_con(rcon, sharpness);
+  return fsr1_upscale_post(&in, &tmp, &out, econ, rcon, post, 0, c->out_h, flags | FSR1_FLAG_FUSED, stream);
 }
 
 int fsr1_context_upscale(fsr1_context* c, const void* in_dev, uint64_t in_pitch, void* out_dev, uint64_t out_pitch,

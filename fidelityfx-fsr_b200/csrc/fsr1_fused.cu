@@ -26,6 +26,7 @@
 // Out-of-image mid pixels hold 0 (D3D12 Load semantics, ffx_fsr1.h:698-707 through FSR_Pass.hlsl:61); FSR1_FLAG_RCAS_CLAMP is not
 // implemented here (the caller falls back to the two-kernel path).
 #include "fsr1_easu_quad.cuh"
+#include "fsr1_post.cuh"
 #include "fsr1_rcas_math.cuh"
 
 namespace fsr1 {
@@ -110,10 +111,12 @@ template <int CY> struct FusedIter {
 // Phase 3 (EASU of the step's cells into the mid tile), a barrier, then RCAS of the step's output rows.  kIn: an interior step
 // (see the caller): no pixel masked, no row skipped, every store a full pair — a predicate-free copy of the body, as
 // easu_h_quad2x_kernel takes for interior tiles.
-template <bool kIn, int NW>
+// SO: void = RCAS's own RGBA16F store; otherwise the display epilogue of fsr1_upscale_post (post_pair, fsr1_post.cuh) with its store.
+template <bool kIn, int NW, typename SO>
 __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams& p, const FusedStep& cur, const uint2* tile, int dx,
-                                           int k0, __half2 sharp, int lane, int warp) {
+                                           int k0, __half2 sharp, int lane, int warp, const PostParams* q) {
   constexpr int CY = FusedCfg<NW>::kCY;
+  constexpr bool kPost = !std::is_void<SO>::value;
   const int n = cur.n;
 #pragma unroll 1
   for (int q = 0; q < 2; q++) {
@@ -136,38 +139,67 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
   const int lm = lane > 0 ? lane - 1 : 0;
   const int ox = 2 * (k0 + lane);  // first pixel of the lane's output pair
   const bool writer = lane >= 1 && (kIn || ox < p.out.w);
-  Row3 E[kR + 2], D[kR], Fv[kR];
+  if constexpr (kPost) {
+    // the epilogue needs registers: a rolling window of three mid rows instead of all kR + 2 up front (no spills at 6 CTAs per SM)
+    auto mid_row = [&](int i, Row3& e, Row3& d, Row3& f) {
+      const uint4 a = sm.mid[i][lm], c = sm.mid[i][lane];
+      e.r = uh2(__byte_perm(a.x, c.x, 0x5432));
+      e.g = uh2(__byte_perm(a.y, c.y, 0x5432));
+      e.b = uh2(__byte_perm(a.z, c.z, 0x5432));
+      d.r = uh2(a.x); d.g = uh2(a.y); d.b = uh2(a.z);
+      f.r = uh2(c.x); f.g = uh2(c.y); f.b = uh2(c.z);
+    };
+    Row3 ea, eb, db, fb, ec, dc, fc;
+    mid_row(i0, ea, dc, fc);
+    mid_row(i0 + 1, eb, db, fb);
+    unsigned char* dst = p.out.base + (long long)(o_first - p.out.row0) * p.out.pitch + (long long)ox * PostStore<SO>::kBytes;
+    PostCursor pc;
+    pc.init(*q, ox, o_first);
 #pragma unroll
-  for (int r = 0; r < kR + 2; r++) {
-    const uint4 a = sm.mid[i0 + r][lm], c = sm.mid[i0 + r][lane];
-    E[r].r = uh2(__byte_perm(a.x, c.x, 0x5432));
-    E[r].g = uh2(__byte_perm(a.y, c.y, 0x5432));
-    E[r].b = uh2(__byte_perm(a.z, c.z, 0x5432));
-    if (r >= 1 && r <= kR) {
-      D[r - 1].r = uh2(a.x); D[r - 1].g = uh2(a.y); D[r - 1].b = uh2(a.z);
-      Fv[r - 1].r = uh2(c.x); Fv[r - 1].g = uh2(c.y); Fv[r - 1].b = uh2(c.z);
+    for (int r = 0; r < kR; r++) {
+      const int o = o_first + r;
+      mid_row(i0 + r + 2, ec, dc, fc);
+      if (kIn || (o >= cur.ya && o < cur.yb && o < 2 * cur.m0 + 2 * n)) {  // warp-uniform
+        __half2 oR, oG, oB;
+        rcas_pair<0>(ea, db, eb, fb, ec, sharp, oR, oG, oB);
+        if (writer) post_pair<SO>(*q, pc, dst + (long long)r * p.out.pitch, ox, o, oR, oG, oB, 0x3c003c00u, kIn || ox + 1 < p.out.w);
+      }
+      pc.next_row(*q);
+      ea = eb; eb = ec; db = dc; fb = fc;
     }
-  }
-  unsigned char* dst = p.out.base + (long long)(o_first - p.out.row0) * p.out.pitch + (long long)ox * 8;
+  } else {
+    Row3 E[kR + 2], D[kR], Fv[kR];
 #pragma unroll
-  for (int r = 0; r < kR; r++) {
-    const int o = o_first + r;
-    if (kIn || (o >= cur.ya && o < cur.yb && o < 2 * cur.m0 + 2 * n)) {  // warp-uniform
-      __half2 oR, oG, oB;
-      rcas_pair<0>(E[r], D[r], E[r + 1], Fv[r], E[r + 2], sharp, oR, oG, oB);
-      if (writer) {
-        const uint4 w = pack_pair_half(oR, oG, oB, 0x3c003c00u);
-        unsigned char* o8 = dst + (long long)r * p.out.pitch;
-        if (kIn || ox + 1 < p.out.w) *reinterpret_cast<uint4*>(o8) = w;
-        else *reinterpret_cast<uint2*>(o8) = make_uint2(w.x, w.y);
+    for (int r = 0; r < kR + 2; r++) {
+      const uint4 a = sm.mid[i0 + r][lm], c = sm.mid[i0 + r][lane];
+      E[r].r = uh2(__byte_perm(a.x, c.x, 0x5432));
+      E[r].g = uh2(__byte_perm(a.y, c.y, 0x5432));
+      E[r].b = uh2(__byte_perm(a.z, c.z, 0x5432));
+      if (r >= 1 && r <= kR) {
+        D[r - 1].r = uh2(a.x); D[r - 1].g = uh2(a.y); D[r - 1].b = uh2(a.z);
+        Fv[r - 1].r = uh2(c.x); Fv[r - 1].g = uh2(c.y); Fv[r - 1].b = uh2(c.z);
+      }
+    }
+    unsigned char* dst = p.out.base + (long long)(o_first - p.out.row0) * p.out.pitch + (long long)ox * 8;
+#pragma unroll
+    for (int r = 0; r < kR; r++) {
+      const int o = o_first + r;
+      if (kIn || (o >= cur.ya && o < cur.yb && o < 2 * cur.m0 + 2 * n)) {  // warp-uniform
+        __half2 oR, oG, oB;
+        rcas_pair<0>(E[r], D[r], E[r + 1], Fv[r], E[r + 2], sharp, oR, oG, oB);
+        if (writer) {
+          const uint4 w = pack_pair_half(oR, oG, oB, 0x3c003c00u);
+          unsigned char* o8 = dst + (long long)r * p.out.pitch;
+          if (kIn || ox + 1 < p.out.w) *reinterpret_cast<uint4*>(o8) = w;
+          else *reinterpret_cast<uint2*>(o8) = make_uint2(w.x, w.y);
+        }
       }
     }
   }
 }
 
-template <int NW, int MINB>
-__global__ void __launch_bounds__(NW * 32, MINB)
-fused_h_quad2x_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap) {
+template <int NW, typename SO>
+__device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMap& tmap, const PostParams* q) {
   using C = FusedCfg<NW>;
   constexpr int NT = NW * 32, CY = C::kCY;
   __shared__ FusedSmem<NW> sm;
@@ -221,8 +253,8 @@ fused_h_quad2x_kernel(const FusedParams p, const __grid_constant__ CUtensorMap t
     // rows lie above ya
     const bool inside = k0 >= 0 && 2 * (k0 + 31) + 2 < p.out.w && cur.m0 >= 0 && 2 * (cur.m0 + CY) < p.out.h && n == CY &&
                         2 * cur.m0 >= cur.ya && 2 * (cur.m0 + CY) <= cur.yb;
-    if (inside) fused_step<true>(sm, p, cur, tile, dx, k0, sharp, lane, warp);
-    else fused_step<false>(sm, p, cur, tile, dx, k0, sharp, lane, warp);
+    if (inside) fused_step<true, NW, SO>(sm, p, cur, tile, dx, k0, sharp, lane, warp, q);
+    else fused_step<false, NW, SO>(sm, p, cur, tile, dx, k0, sharp, lane, warp, q);
     __syncthreads();
     if (n == CY && tid < 64) {  // the run may continue: its last two mid rows become rows 0, 1 of the next step
       const int rr = tid >> 5;
@@ -236,17 +268,32 @@ fused_h_quad2x_kernel(const FusedParams p, const __grid_constant__ CUtensorMap t
   halo_sync_end(p.sync);
 }
 
+template <int NW, int MINB>
+__global__ void __launch_bounds__(NW * 32, MINB)
+fused_h_quad2x_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap) {
+  fused_body<NW, void>(p, tmap, nullptr);
+}
+
+// fsr1_upscale_post: the same kernel with the display epilogue in RCAS's store (SO: __half, Unorm8, Unorm10)
+template <int NW, int MINB, typename SO>
+__global__ void __launch_bounds__(NW * 32, MINB)
+fused_h_quad2x_post_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap, const __grid_constant__ PostParams q) {
+  fused_body<NW, SO>(p, tmap, &q);
+}
+
 #ifndef FSR1_CPU_EMU
-cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name) {
-  if (clamp) return cudaErrorNotSupported;
+// tensor map, parameters and grid of a fused launch; cudaErrorNotSupported when the frame is not one the kernel takes.
+// out_align: the alignment the output store needs (16 for RGBA16F pairs, 8 for UNORM pairs).
+static cudaError_t fused_setup(const EasuParams& e, uint32_t sharp_h2, int out_align, CUtensorMap& tmap, FusedParams& p, int& per_sm,
+                               long long& grid) {
   if (!(e.c0x == 0.5f && e.c0y == 0.5f && e.c0z == -0.25f && e.c0w == -0.25f)) return cudaErrorNotSupported;
-  if ((reinterpret_cast<uintptr_t>(e.in.base) & 15) || (e.in.pitch & 15) || (reinterpret_cast<uintptr_t>(e.out.base) & 15) || (e.out.pitch & 15))
+  if ((reinterpret_cast<uintptr_t>(e.in.base) & 15) || (e.in.pitch & 15) || (reinterpret_cast<uintptr_t>(e.out.base) & (out_align - 1)) ||
+      (e.out.pitch & (out_align - 1)))
     return cudaErrorNotSupported;
   constexpr int NW = 4;
   using C = FusedCfg<NW>;
   EncodeTiledFn encode = get_encode_fn();
   if (!encode) return cudaErrorNotSupported;
-  CUtensorMap tmap;
   const cuuint64_t dims[2] = {(cuuint64_t)e.in.w, (cuuint64_t)e.in.rows};
   const cuuint64_t strides[1] = {(cuuint64_t)e.in.pitch};
   const cuuint32_t box[2] = {(cuuint32_t)kFBW, (cuuint32_t)C::kBH};
@@ -254,19 +301,58 @@ cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cu
   if (encode(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, e.in.base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
     return cudaErrorNotSupported;
-  FusedParams p;
   p.in = e.in; p.out = e.out; p.y0 = e.y0; p.y1 = e.y1; p.sharp_h2 = sharp_h2; p.sync = e.sync;
   // output pairs (2k, 2k+1), k = 0 .. (w-1)/2, 31 per strip
   p.n_strips = ((e.out.w + 1) / 2 + kStripCells - 1) / kStripCells;
   const long long units = (long long)p.n_strips * ((e.y1 - e.y0 + 1) / 2);
   // 72 registers = 7 CTAs per SM, as easu_h_quad2x; a launch that waits for a neighbour's halo (p.sync) takes 6 so that the
   // one-warp halo_push_kernel it waits for still fits beside it (launch_easu_h_tiled, DESIGN.md §6)
-  const int per_sm = (p.sync.ready[0] || p.sync.ready[1]) ? 6 : 7;
-  long long grid = (long long)per_sm * sm_count();
+  if (p.sync.ready[0] || p.sync.ready[1]) per_sm = 6;
+  grid = (long long)per_sm * sm_count();
   if (grid > (units + 7) / 8) grid = (units + 7) / 8;  // at least ~16 rows of a strip per CTA
   if (grid < 1) grid = 1;
-  fused_h_quad2x_kernel<NW, 7><<<(int)grid, NW * 32, 0, s>>>(p, tmap);
+  return cudaSuccess;
+}
+
+cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name) {
+  if (clamp) return cudaErrorNotSupported;
+  CUtensorMap tmap;
+  FusedParams p;
+  int per_sm = 7;
+  long long grid = 0;
+  const cudaError_t err = fused_setup(e, sharp_h2, 16, tmap, p, per_sm, grid);
+  if (err != cudaSuccess) return err;
+  fused_h_quad2x_kernel<4, 7><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
   *name = per_sm == 7 ? "fused_easu_rcas_h_quad2x<4w,7/sm,tma2,strips>" : "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips>";
+  return cudaGetLastError();
+}
+
+// The display epilogue needs more registers than the 72 of 7 CTAs per SM (-Xptxas -v: DESIGN.md §4): 6 per SM.
+constexpr int kPostPerSm = 6;
+
+cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const PostParams& q, int out_format, cudaStream_t s,
+                                const char** name) {
+  CUtensorMap tmap;
+  FusedParams p;
+  int per_sm = kPostPerSm;
+  long long grid = 0;
+  const cudaError_t err = fused_setup(e, sharp_h2, out_format == 1 ? 16 : 8, tmap, p, per_sm, grid);
+  if (err != cudaSuccess) return err;
+  switch (out_format) {
+    case 1:
+      fused_h_quad2x_post_kernel<4, kPostPerSm, __half><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f>";
+      break;
+    case 3:
+      fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm8><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8>";
+      break;
+    case 4:
+      fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm10><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2>";
+      break;
+    default: return cudaErrorNotSupported;
+  }
   return cudaGetLastError();
 }
 #endif

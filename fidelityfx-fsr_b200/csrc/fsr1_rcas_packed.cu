@@ -15,6 +15,7 @@
 // UNORM texels are decoded to the same (pixel0, pixel1)-per-channel half2 form (c / (2^n - 1) in fp32, one rounding to
 // half) and the saturated result is re-encoded in the half domain (x * (2^n - 1) + 1024 leaves round(x * (2^n - 1)) in the
 // low mantissa bits).
+#include "fsr1_post.cuh"
 #include "fsr1_rcas_math.cuh"
 
 namespace fsr1 {
@@ -116,8 +117,11 @@ __device__ __forceinline__ typename FM::Raw load_checked(const RcasParams& p, in
                     x + 1 >= 0 && x + 1 < p.in.w ? row + (long long)(x + 1) * FM::kBpp : nullptr);
 }
 
-template <typename FM, bool kChecked, bool kClamp, int kOpt>
-__device__ __forceinline__ void rcas_rows(const RcasParams& p, int x, int ys, int lane) {
+// SO: void = FM's own store; otherwise the display epilogue of fsr1_upscale_post (post_pair, fsr1_post.cuh) with its store.
+template <typename FM, bool kChecked, bool kClamp, int kOpt, typename SO = void>
+__device__ __forceinline__ void rcas_rows(const RcasParams& p, int x, int ys, int lane, const PostParams* q = nullptr) {
+  constexpr bool kPost = !std::is_void<SO>::value;
+  constexpr int kOutBpp = kPost ? PostStore<SO>::kBytes : FM::kBpp;
   const __half2 sharp = uh2(p.sharp_h2);
   const bool writer = lane >= 1 && lane <= 30 && (!kChecked || x < p.out.w);
   // all kRows+2 rows are requested up front: kRows+2 independent vector loads in flight per lane
@@ -139,7 +143,9 @@ __device__ __forceinline__ void rcas_rows(const RcasParams& p, int x, int ys, in
       if ((kOpt & kRcasAlpha) && r >= 1 && r <= kRows) alphas[r - 1] = FM::alpha(v);
     }
   }
-  unsigned char* dst = p.out.base + (long long)(ys - p.out.row0) * p.out.pitch + (long long)x * FM::kBpp;
+  unsigned char* dst = p.out.base + (long long)(ys - p.out.row0) * p.out.pitch + (long long)x * kOutBpp;
+  PostCursor pc;
+  if constexpr (kPost) pc.init(*q, x, ys);
 #pragma unroll
   for (int r = 0; r < kRows; r++) {
     const int y = ys + r;
@@ -155,8 +161,14 @@ __device__ __forceinline__ void rcas_rows(const RcasParams& p, int x, int ys, in
     f.b = uh2(__byte_perm(hu2(cur.b), __shfl_down_sync(0xffffffffu, hu2(cur.b), 1), 0x5432));
     __half2 oR, oG, oB;
     rcas_pair<kOpt>(prev, d, cur, f, next, sharp, oR, oG, oB);
-    if (writer)
+    if constexpr (kPost) {
+      if (writer)
+        post_pair<SO>(*q, pc, dst + (long long)r * p.out.pitch, x, y, oR, oG, oB, (kOpt & kRcasAlpha) ? alphas[r] : FM::opaque(),
+                      !kChecked || x + 1 < p.out.w);
+      pc.next_row(*q);
+    } else if (writer) {
       FM::store(dst + (long long)r * p.out.pitch, oR, oG, oB, (kOpt & kRcasAlpha) ? alphas[r] : FM::opaque(), !kChecked || x + 1 < p.out.w);
+    }
   }
 }
 
@@ -172,6 +184,21 @@ __global__ void __launch_bounds__(32 * kNW) rcas_packed_kernel(const RcasParams 
     rcas_rows<FM, false, kClamp, kOpt>(p, x, ys, lane);
   else
     rcas_rows<FM, true, kClamp, kOpt>(p, x, ys, lane);
+}
+
+// fsr1_upscale_post: RCAS of an RGBA16F intermediate with the display epilogue in the store (SO: __half, Unorm8, Unorm10)
+template <bool kClamp, int kOpt, typename SO>
+__global__ void __launch_bounds__(32 * kNW) rcas_post_kernel(const RcasParams p, const __grid_constant__ PostParams q) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int x0 = blockIdx.x * kSpan - 2;
+  const int x = x0 + lane * 2;
+  const int ys = p.y0 + (blockIdx.y * kNW + warp) * kRows;
+  if (ys >= p.y1) return;  // whole warp
+  const bool interior = x0 >= 0 && x0 + 64 <= p.in.w && ys >= 1 && ys + kRows < p.in.h && ys + kRows <= p.y1;
+  if (interior)
+    rcas_rows<FmtHalf, false, kClamp, kOpt, SO>(p, x, ys, lane, &q);
+  else
+    rcas_rows<FmtHalf, true, kClamp, kOpt, SO>(p, x, ys, lane, &q);
 }
 
 #ifndef FSR1_CPU_EMU  // tests/emu compiles the device code above for the host and supplies its own launcher
@@ -209,6 +236,41 @@ cudaError_t launch_rcas_u_packed(const RcasParams& p, int format, cudaStream_t s
   if (format != 3 || !aligned(p, 8)) return cudaErrorNotSupported;
   *name = "rcas_u8_packed<2px,4rows,shfl60>";
   return launch_fmt<FmtUnorm<8>>(p, s);
+}
+
+template <typename SO, bool kClamp>
+static void launch_post_opt(const RcasParams& p, const PostParams& q, dim3 grid, cudaStream_t s) {
+  switch (p.options & 7) {
+    case 0: rcas_post_kernel<kClamp, 0, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 1: rcas_post_kernel<kClamp, 1, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 2: rcas_post_kernel<kClamp, 2, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 3: rcas_post_kernel<kClamp, 3, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 4: rcas_post_kernel<kClamp, 4, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 5: rcas_post_kernel<kClamp, 5, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 6: rcas_post_kernel<kClamp, 6, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    default: rcas_post_kernel<kClamp, 7, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+  }
+}
+template <typename SO>
+static cudaError_t launch_post_fmt(const RcasParams& p, const PostParams& q, cudaStream_t s) {
+  const dim3 grid((p.out.w + kSpan - 1) / kSpan, (p.y1 - p.y0 + kNW * kRows - 1) / (kNW * kRows), 1);
+  if (p.clamp) launch_post_opt<SO, true>(p, q, grid, s);
+  else launch_post_opt<SO, false>(p, q, grid, s);
+  return cudaGetLastError();
+}
+
+// p.in: the RGBA16F intermediate; p.out: RGBA16F (out_format 1), RGBA8_UNORM (3) or RGB10A2_UNORM (4)
+cudaError_t launch_rcas_h_post(const RcasParams& p, const PostParams& q, int out_format, cudaStream_t s, const char** name) {
+  const int oa = out_format == 1 ? 16 : 8;
+  if ((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15) || (reinterpret_cast<uintptr_t>(p.out.base) & (oa - 1)) ||
+      (p.out.pitch & (oa - 1)))
+    return cudaErrorNotSupported;
+  switch (out_format) {
+    case 1: *name = "rcas_h_packed_post<2px,4rows,shfl60,rgba16f>"; return launch_post_fmt<__half>(p, q, s);
+    case 3: *name = "rcas_h_packed_post<2px,4rows,shfl60,rgba8>"; return launch_post_fmt<Unorm8>(p, q, s);
+    case 4: *name = "rcas_h_packed_post<2px,4rows,shfl60,rgb10a2>"; return launch_post_fmt<Unorm10>(p, q, s);
+  }
+  return cudaErrorNotSupported;
 }
 
 cudaError_t launch_rcas_h_packed(const RcasParams& p, cudaStream_t s, const char** name) {

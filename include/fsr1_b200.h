@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h */
+#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post */
 
 enum {
   FSR1_OK = 0,
@@ -232,6 +232,42 @@ int fsr1_lfga_h(const fsr1_image* in, const fsr1_image* grain, const fsr1_image*
                 uint32_t y1, void* stream);
 int fsr1_tepd_h(const fsr1_image* in, const fsr1_image* dither, const fsr1_image* out, int bits, uint32_t frame,
                 uint32_t y0, uint32_t y1, void* stream);
+
+/* ---- upscale straight to the display output (ffx_fsr1.h:1030-1040 usage notes) ------------------
+ * fsr1_upscale followed by the passes an application runs after RCAS, applied inside RCAS's store instead of as whole-image passes:
+ * the chain writes the output once and reads nothing extra but the small grain / dither tiles.  The result is bit-identical, on rows
+ * [y0, y1), to
+ *     fsr1_upscale(in, tmp, T, easu_con, rcas_con, y0, y1, flags)      T: an RGBA16F image of out's size
+ *     FSR1_POST_SRTM_INVERSE:  fsr1_srtm(T, T, 1, ...)                 FsrSrtmInvF      ffx_fsr1.h:1046
+ *     FSR1_POST_LFGA:          fsr1_lfga(T, grain, T, lfga_amount, ...) FsrLfgaF        ffx_fsr1.h:1014
+ *     FSR1_POST_TEPD8 / 10:    fsr1_tepd(T, dither, out, 8 / 10, frame, ...)  FsrTepdC8F / C10F  ffx_fsr1.h:1100-1126
+ * in that order (the last step writes `out`).  Alpha is what RCAS stores (1, or the input's with FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA).
+ *   in      RGBA16F.
+ *   out     RGBA16F; with TEPD also RGBA8_UNORM (TEPD8) or RGB10A2_UNORM (TEPD10): the code values, as fsr1_tepd writes them.
+ *   tmp     the RGBA16F intermediate of the two-kernel path (as fsr1_upscale); NULL is accepted when the frame takes the fused
+ *           kernel (FSR1_FLAG_FUSED, exactly 2x, no RCAS option, no OUTPUT_SQUARE, no PRECISE), which then is the only launch.
+ *   post    NULL or ops == 0: exactly fsr1_upscale.  grain: an RGBA16F / RGBA32F tile (wrap addressing, as fsr1_lfga); dither:
+ *           NULL = FsrTepdDitF(pixel, frame), else the saturated .w of a tile (as fsr1_tepd).  Tiles are whole images.
+ * Every other scale, the RCAS options, OUTPUT_SQUARE and PRECISE run EASU into tmp and one RCAS kernel with the epilogue.
+ * FSR1_ERR_UNSUPPORTED: another input/output format, FSR1_FLAG_EXACT / FORCE_DIRECT / H_REFERENCE / RCAS_HX2 / NO_RCAS, or a layout
+ * the packed kernels cannot take (out and tmp 16-byte aligned, 8 for UNORM out); those callers keep using the separate passes.
+ * FSR1_ERR_INVALID_ARGUMENT: unknown ops bits, both TEPD bits, LFGA without a grain tile, a tile that is a window.  All
+ * validation happens before any CUDA call. */
+enum { FSR1_POST_SRTM_INVERSE = 1u << 0, FSR1_POST_LFGA = 1u << 1, FSR1_POST_TEPD8 = 1u << 2, FSR1_POST_TEPD10 = 1u << 3 };
+typedef struct fsr1_post {
+  uint32_t ops;              /* FSR1_POST_*, applied in this order; TEPD8 and TEPD10 exclusive */
+  float lfga_amount;
+  const fsr1_image* grain;   /* LFGA tile */
+  const fsr1_image* dither;  /* TEPD tile or NULL */
+  uint32_t frame, reserved;  /* TEPD positional dither: FsrTepdDitF(pixel, frame) */
+} fsr1_post;
+int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, const uint32_t easu_con[16],
+                      const uint32_t rcas_con[4], const fsr1_post* post, uint32_t y0, uint32_t y1, uint32_t flags, void* stream);
+/* The context form, as fsr1_context_upscale_render (render size 0 = the context's input size; always FSR1_FLAG_FUSED).  The context's
+ * format must be RGBA16F.  `out_dev` is RGBA8_UNORM with TEPD8, RGB10A2_UNORM with TEPD10, RGBA16F otherwise. */
+int fsr1_context_upscale_post(fsr1_context* ctx, const void* in_dev, uint64_t in_pitch, uint32_t render_width,
+                              uint32_t render_height, void* out_dev, uint64_t out_pitch, float sharpness_stops,
+                              const fsr1_post* post, uint32_t flags, void* stream);
 
 /* ---- constants through the ABI (for FFIs that cannot include fsr1_host.h) ---------------------- */
 void fsr1_easu_con(uint32_t con[16], float in_viewport_w, float in_viewport_h, float in_size_w, float in_size_h,
