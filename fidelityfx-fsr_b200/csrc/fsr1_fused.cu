@@ -14,9 +14,9 @@
 // The result is bit-identical to fsr1_easu + fsr1_rcas (tests/test_gpu_parity.py::test_fused_*): same operations on the same
 // rounded intermediate.  Compulsory HBM traffic: bpp (Pin + Pout) = 10 B per output pixel instead of 26.
 //
-// Work distribution: the image is n_strips x rows; in a linear order (strip-major, units of two rows) CTA c takes the c-th
-// of gridDim.x equal shares, i.e. 1-2 "runs" (strip, [ya, yb)).  A run starts like a row slab: its first step also computes the
-// cell row above ya (RCAS's upper neighbour), which is the only vertical redundancy (~1 cell row per ~65).
+// Work distribution (FusedIter): the CTAs of a strip split it into "runs" (strip, [ya, yb)) of whole steps.  A run starts like
+// a row slab: its first step also computes the cell row above ya (RCAS's upper neighbour), which is the only vertical
+// redundancy (~1 cell row per ~73 at 1080p->4K).  Only a strip's last run may end with a partial step.
 //
 // Geometry of a step with cell rows m0 .. m0+n-1 (n <= CY) of strip tx (cells k0 .. k0+31, k0 = 31 tx - 1):
 //   mid row index i  <->  pixel row 2 m0 - 1 + i   (i = 0, 1: kept from the previous step; cell row r -> i = 2r+2, 2r+3)
@@ -75,42 +75,57 @@ template <bool kIn> struct MidSink {
 
 struct FusedStep { int tx, m0, n, ya, yb; };
 
-// the CTA's share of the (strip, row-pair) space, cut into runs and steps
+// The CTA's share of the work, in whole steps of CY cell rows of one strip.  A strip needs cell rows mfirst .. mlast (pixel rows
+// y0 - 1 .. y1).  With at least as many CTAs as strips, strip s goes to the g CTAs [ctas s / S, ctas (s+1) / S); they split it into
+// runs of whole steps, and a run's first cell row is the last one of the run above (the upper neighbour of its first output row),
+// so g runs cover the C = mlast - mfirst + 1 cell rows in T = ceil((C + g - 1) / CY) steps and CTA i of the g takes steps
+// [T i / g, T (i+1) / g).  Only the strip's last run may end with a partial step, at y1.  (When T < g, some CTAs take no step and
+// the T runs of one step each overlap T - 1 times: T = ceil((C - 1) / (CY - 1)).)  With fewer CTAs than strips a CTA takes whole
+// strips.  A run's first step produces the output rows of its last CY - 1 cell rows, every later step those of all CY.
 template <int CY> struct FusedIter {
-  long long pos, hi;
-  int rows2, y0, y1;
-  int strip, ya, yb, m, mend;
+  int y0, y1, mfirst, mlast;
+  int strip, strip_end, ma, mb, m;
   __device__ void init(const FusedParams& p, int cta, int ctas) {
     y0 = p.y0; y1 = p.y1;
-    rows2 = (p.y1 - p.y0 + 1) >> 1;
-    const long long total = (long long)p.n_strips * rows2;
-    pos = total * cta / ctas;
-    hi = total * (cta + 1) / ctas;
-    m = 0; mend = -1; strip = 0; ya = yb = 0;
+    mfirst = (y0 - 2) >> 1;  // cell row holding pixel row y0-1 (arithmetic shift = floor)
+    mlast = (y1 - 1) >> 1;   // cell row holding pixel row y1
+    const int S = p.n_strips, C = mlast - mfirst + 1;
+    strip = strip_end = 0; ma = 0; mb = -1; m = 1;
+    if (y1 <= y0) return;
+    if (ctas < S) {
+      strip = (int)((long long)S * cta / ctas);
+      strip_end = (int)((long long)S * (cta + 1) / ctas);
+      ma = mfirst; mb = mlast; m = ma;
+      return;
+    }
+    const int s = (int)(((long long)(cta + 1) * S - 1) / ctas);
+    const int g0 = (int)((long long)ctas * s / S), g = (int)((long long)ctas * (s + 1) / S) - g0, i = cta - g0;
+    int T = (C + g - 1 + CY - 1) / CY;
+    if (T < g) T = (C - 1 + CY - 2) / (CY - 1);
+    const int a = (int)((long long)T * i / g), k = (int)((long long)T * (i + 1) / g) - a;
+    const int ra = mfirst + CY * a - (i < a ? i : a);  // each run above this one (min(i, a) of them) shares a cell row with the next
+    if (k == 0 || 2 * ra + 2 >= y1) return;            // no step, or the runs above already cover the strip
+    ma = ra;
+    mb = ma + CY * k - 1 < mlast ? ma + CY * k - 1 : mlast;
+    strip = s; strip_end = s + 1; m = ma;
   }
   __device__ bool next(FusedStep& s) {
-    if (m > mend) {  // next run
-      if (pos >= hi) return false;
-      strip = (int)(pos / rows2);
-      const int a2 = (int)(pos - (long long)strip * rows2);
-      const long long left = hi - pos, room = rows2 - a2;
-      const int take = (int)(left < room ? left : room);
-      ya = y0 + 2 * a2;
-      yb = ya + 2 * take < y1 ? ya + 2 * take : y1;
-      pos += take;
-      m = (ya - 2) >> 1;     // cell row holding pixel row ya-1 (arithmetic shift = floor)
-      mend = (yb - 1) >> 1;  // cell row holding pixel row yb
+    if (m > mb) {  // next strip (fewer CTAs than strips)
+      if (++strip >= strip_end) return false;
+      m = ma;
     }
-    s.tx = strip; s.m0 = m; s.ya = ya; s.yb = yb;
-    s.n = mend - m + 1 < CY ? mend - m + 1 : CY;
+    s.tx = strip; s.m0 = m;
+    s.ya = 2 * ma + 2 > y0 ? 2 * ma + 2 : y0;
+    s.yb = 2 * mb + 2 < y1 ? 2 * mb + 2 : y1;
+    s.n = mb - m + 1 < CY ? mb - m + 1 : CY;
     m += s.n;
     return true;
   }
 };
 
 // Phase 3 (EASU of the step's cells into the mid tile), a barrier, then RCAS of the step's output rows.  kIn: an interior step
-// (see the caller): no pixel masked, no row skipped, every store a full pair — a predicate-free copy of the body, as
-// easu_h_quad2x_kernel takes for interior tiles.
+// (see the caller): no pixel masked, every store a full pair, no row skipped but the first two of a run's first step — a
+// predicate-free copy of the body, as easu_h_quad2x_kernel takes for interior tiles.
 // SO: void = RCAS's own RGBA16F store; otherwise the display epilogue of fsr1_upscale_post (post_pair, fsr1_post.cuh) with its store.
 template <bool kIn, int NW, typename SO>
 __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams& p, const FusedStep& cur, const uint2* tile, int dx,
@@ -139,6 +154,8 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
   const int lm = lane > 0 ? lane - 1 : 0;
   const int ox = 2 * (k0 + lane);  // first pixel of the lane's output pair
   const bool writer = lane >= 1 && (kIn || ox < p.out.w);
+  // kIn: only the first two rows of a run's first step (warp 0) lie above ya; they are computed like the others, not stored
+  const bool wtop = writer && (!kIn || o_first >= cur.ya);
   if constexpr (kPost) {
     // the epilogue needs registers: a rolling window of three mid rows instead of all kR + 2 up front (no spills at 6 CTAs per SM)
     auto mid_row = [&](int i, Row3& e, Row3& d, Row3& f) {
@@ -162,7 +179,7 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
       if (kIn || (o >= cur.ya && o < cur.yb && o < 2 * cur.m0 + 2 * n)) {  // warp-uniform
         __half2 oR, oG, oB;
         rcas_pair<0>(ea, db, eb, fb, ec, sharp, oR, oG, oB);
-        if (writer) post_pair<SO>(*q, pc, dst + (long long)r * p.out.pitch, ox, o, oR, oG, oB, 0x3c003c00u, kIn || ox + 1 < p.out.w);
+        if (r >= 2 ? writer : wtop) post_pair<SO>(*q, pc, dst + (long long)r * p.out.pitch, ox, o, oR, oG, oB, 0x3c003c00u, kIn || ox + 1 < p.out.w);
       }
       pc.next_row(*q);
       ea = eb; eb = ec; db = dc; fb = fc;
@@ -187,7 +204,7 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
       if (kIn || (o >= cur.ya && o < cur.yb && o < 2 * cur.m0 + 2 * n)) {  // warp-uniform
         __half2 oR, oG, oB;
         rcas_pair<0>(E[r], D[r], E[r + 1], Fv[r], E[r + 2], sharp, oR, oG, oB);
-        if (writer) {
+        if (r >= 2 ? writer : wtop) {
           const uint4 w = pack_pair_half(oR, oG, oB, 0x3c003c00u);
           unsigned char* o8 = dst + (long long)r * p.out.pitch;
           if (kIn || ox + 1 < p.out.w) *reinterpret_cast<uint4*>(o8) = w;
@@ -249,10 +266,10 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
     }
     __syncthreads();
     // interior step: the strip's cells and pixels are in the image (k0 >= 0, m0 >= 0, last pixel column and row inside), the step
-    // is full (n = CY) and every output row it produces lies in [ya, yb) — never the first step of a run, whose first two output
-    // rows lie above ya
+    // is full (n = CY) and every output row it produces lies in [ya, yb), but for the first two of a run's first step, which lie
+    // above ya (fused_step skips them)
     const bool inside = k0 >= 0 && 2 * (k0 + 31) + 2 < p.out.w && cur.m0 >= 0 && 2 * (cur.m0 + CY) < p.out.h && n == CY &&
-                        2 * cur.m0 >= cur.ya && 2 * (cur.m0 + CY) <= cur.yb;
+                        2 * cur.m0 + 2 >= cur.ya && 2 * (cur.m0 + CY) <= cur.yb;
     if (inside) fused_step<true, NW, SO>(sm, p, cur, tile, dx, k0, sharp, lane, warp, q);
     else fused_step<false, NW, SO>(sm, p, cur, tile, dx, k0, sharp, lane, warp, q);
     __syncthreads();
