@@ -37,6 +37,19 @@ def expected_easu_kernel(con, fmt, flags=0):
     return "easu_direct"
 
 
+def viewport_2x(n, con_of):
+    """A viewport for an output n pixels long whose constants are exactly 2x: n / 2, or the float32 nearest to it for which
+    FsrEasuCon's n / 2 * rcp(n) rounds to 0.5 (for n = 61 it gives 0.49999997), so that odd outputs take the 2x kernels.
+    con_of(v, n): the constant block of a v x v viewport scaled to n x n."""
+    up = dn = np.float32(n / 2.0)
+    for _ in range(16):
+        for v in (up, dn):
+            if con_of(float(v), n)[:4:2] == _QUAD_2X[:4:2]:
+                return float(v)
+        up, dn = np.nextafter(up, np.float32(np.inf)), np.nextafter(dn, np.float32(0))
+    raise AssertionError("no exact 2x viewport for %d" % n)
+
+
 def cells(n_out, scale_word, offset_word):
     """Cell index of each output pixel along one axis, in the fp32 arithmetic of host_cell (csrc/fsr1_capi.cu): one rounding
     per operation, no fused multiply-add."""
