@@ -9,7 +9,7 @@ import torch
 
 from . import _lib
 from ._lib import FORMAT_RGB10A2_UNORM, FORMAT_RGBA8_UNORM  # noqa: F401
-from ._lib import FLAG_FUSED, FLAG_OUTPUT_SQUARE, FLAG_RCAS_HX2  # noqa: F401
+from ._lib import FLAG_FUSED, FLAG_OUTPUT_SQUARE, FLAG_RCAS_HX2, FLAG_SRTM_INPUT  # noqa: F401
 from ._lib import POST_LFGA, POST_SRTM_INVERSE, POST_TEPD10, POST_TEPD8  # noqa: F401
 from ._lib import (FLAG_EXACT, FLAG_FORCE_DIRECT, FLAG_H_REFERENCE, FLAG_NO_RCAS, FLAG_PRECISE, FLAG_RCAS_DENOISE, FLAG_RCAS_PASSTHROUGH_ALPHA, FLAG_RCAS_CLAMP, FORMAT_RGBA16F,  # noqa: F401
                    FORMAT_RGBA32F, Fsr1Error, Image)
@@ -203,7 +203,7 @@ class FramePipeline:
         self._L = _lib.lib()
         self._econ, self._rcon = (ctypes.c_uint32 * 16)(*econ), (ctypes.c_uint32 * 4)(*rcon)
         self._imgs = [(_as_img(a), _as_img(t), _as_img(b)) for a, t, b in sets]
-        self._flags = flags
+        self._rcas_flags = flags & ~FLAG_SRTM_INPUT         # the input tonemap belongs to EASU's loads only
         self._easu_flags = flags & ~FLAG_OUTPUT_SQUARE      # the Sample.x hook belongs to the LAST pass only
         if priorities is None:
             self.stream_easu, self.stream_rcas = torch.cuda.Stream(device=device), torch.cuda.Stream(device=device)
@@ -230,7 +230,7 @@ class FramePipeline:
             _lib.check(rc)
         self._easu_done[slot].record(sa)
         sb.wait_event(self._easu_done[slot])
-        rc = self._L.fsr1_rcas(ctypes.byref(t), ctypes.byref(b), self._rcon, self._rrows[0], self._rrows[1], self._flags,
+        rc = self._L.fsr1_rcas(ctypes.byref(t), ctypes.byref(b), self._rcon, self._rrows[0], self._rrows[1], self._rcas_flags,
                                ctypes.c_void_p(sb.cuda_stream))
         if rc:
             _lib.check(rc)

@@ -84,10 +84,24 @@ float as_float(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
 // every flag include/fsr1_b200.h defines
 constexpr uint32_t kAllFlags = FSR1_FLAG_RCAS_CLAMP | FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_NO_RCAS |
                                FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_DENOISE |
-                               FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA | FSR1_FLAG_OUTPUT_SQUARE | FSR1_FLAG_FUSED | FSR1_FLAG_RCAS_HX2;
+                               FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA | FSR1_FLAG_OUTPUT_SQUARE | FSR1_FLAG_FUSED | FSR1_FLAG_RCAS_HX2 |
+                               FSR1_FLAG_SRTM_INPUT;
 
 bool window_holds(const fsr1_image* im, int first, int last) {  // logical rows [first,last]
   return first >= (int)im->row0 && last < (int)(im->row0 + im->rows);
+}
+
+// FSR1_FLAG_SRTM_INPUT: only the TMA-tiled RGBA16F EASU kernels (and the fused kernels built on them) apply FsrSrtmF as they load,
+// so everything those kernels decline is refused here, before any CUDA call, instead of falling back to a kernel that would ignore
+// the flag.  `out`: the image EASU writes (the intermediate, or the output of a fused frame); null when not checked here.
+int srtm_input_check(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], uint32_t flags) {
+  if (in->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
+  if (flags & (FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE)) return FSR1_ERR_UNSUPPORTED;
+  if (((uintptr_t)in->data & 15) || (in->pitch_bytes & 15)) return FSR1_ERR_UNSUPPORTED;  // TMA
+  if (out && (((uintptr_t)out->data & 15) || (out->pitch_bytes & 15))) return FSR1_ERR_UNSUPPORTED;  // 16-byte pixel-pair stores
+  const float sx = as_float(con[0]), sy = as_float(con[1]);
+  if (!(sx > 0.0f && sx <= 1.0f && sy > 0.0f && sy <= 1.0f)) return FSR1_ERR_UNSUPPORTED;  // upscaling only
+  return FSR1_OK;
 }
 
 // the Sample.x hook: `c *= c` in place on the rows the last pass wrote (a separate streaming pass)
@@ -205,6 +219,8 @@ int fsr1_easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16
   uint32_t r0, r1;
   fsr1_easu_input_rows(con, in->height, y0, y1, &r0, &r1);
   if (!window_holds(in, (int)r0, (int)r1)) return FSR1_ERR_WINDOW;
+  const bool srtm_in = (flags & FSR1_FLAG_SRTM_INPUT) != 0;
+  if (srtm_in && (rc = srtm_input_check(in, out, con, flags)) != FSR1_OK) return rc;
 
   EasuParams p;
   p.in = view_of(in);
@@ -222,10 +238,11 @@ int fsr1_easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16
     if (flags & FSR1_FLAG_PRECISE) e = launch_easu_h_precise(p, s, &name);
     if (e == cudaErrorNotSupported) {
       if (t_sync) p.sync = *t_sync;  // sharded frame: the neighbour hand-shake rides inside the kernel
-      e = launch_easu_h_tiled(p, s, &name);
+      e = launch_easu_h_tiled(p, s, &name, srtm_in);
       if (e == cudaSuccess && t_sync) t_sync_used = true;
       p.sync = HaloSync{};
     }
+    if (e == cudaErrorNotSupported && srtm_in) return FSR1_ERR_UNSUPPORTED;  // nothing launched; no other kernel applies the flag
   } else if (in->format == FSR1_FORMAT_RGBA32F && !exact && !(flags & FSR1_FLAG_FORCE_DIRECT)) {
     e = launch_easu_f32_tiled(p, s, &name);
   } else if ((in->format == FSR1_FORMAT_RGBA8_UNORM || in->format == FSR1_FORMAT_RGB10A2_UNORM) && !exact &&
@@ -246,6 +263,7 @@ int fsr1_rcas(const fsr1_image* in, const fsr1_image* out, const uint32_t con[4]
   int rc;
   if ((rc = check_image(in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
   if (!con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
+  if (flags & FSR1_FLAG_SRTM_INPUT) return FSR1_ERR_INVALID_ARGUMENT;  // RCAS has no input stage
   if (in->format != out->format) return FSR1_ERR_UNSUPPORTED;
   if (in->width != out->width || in->height != out->height) return FSR1_ERR_INVALID_ARGUMENT;
   if (y1 == 0) y1 = out->height;
@@ -321,6 +339,8 @@ int fsr1_upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
     uint32_t r0, r1;
     fsr1_easu_input_rows(easu_con, in->height, e0, e1, &r0, &r1);
     if (!window_holds(in, (int)r0, (int)r1)) return FSR1_ERR_WINDOW;
+    const bool srtm_in = (flags & FSR1_FLAG_SRTM_INPUT) != 0;
+    if (srtm_in && (rc = srtm_input_check(in, nullptr, easu_con, flags)) != FSR1_OK) return rc;
     EasuParams p;
     p.in = view_of(in);
     p.out = view_of(out);
@@ -328,7 +348,7 @@ int fsr1_upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
     p.y0 = (int)y0; p.y1 = (int)y1;
     const char* name = "";
     if (t_sync) p.sync = *t_sync;
-    const cudaError_t e = launch_fused_h(p, rcas_con[1], 0, static_cast<cudaStream_t>(stream), &name);
+    const cudaError_t e = launch_fused_h(p, rcas_con[1], 0, static_cast<cudaStream_t>(stream), &name, srtm_in);
     if (e == cudaSuccess && t_sync) t_sync_used = true;
     if (e == cudaSuccess) {
       t_last_kernel = name;
@@ -341,7 +361,7 @@ int fsr1_upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
   if (!tmp) return FSR1_ERR_INVALID_ARGUMENT;
   int rc = fsr1_easu(in, tmp, easu_con, e0, e1, flags & ~(uint32_t)FSR1_FLAG_OUTPUT_SQUARE, stream);  // last pass only
   if (rc != FSR1_OK) return rc;
-  return fsr1_rcas(tmp, out, rcas_con, y0, y1, flags, stream);
+  return fsr1_rcas(tmp, out, rcas_con, y0, y1, flags & ~(uint32_t)FSR1_FLAG_SRTM_INPUT, stream);  // EASU's load stage only
 }
 
 // ---- upscale straight to the display output ----------------------------------------------------------------
@@ -388,6 +408,8 @@ int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_im
   // the half-arithmetic parity paths, fp32 EXACT/direct kernels and EASU-only frames keep the separate passes
   if (flags & (FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_RCAS_HX2 | FSR1_FLAG_NO_RCAS))
     return FSR1_ERR_UNSUPPORTED;
+  const bool srtm_in = (flags & FSR1_FLAG_SRTM_INPUT) != 0;
+  if (srtm_in && (rc = srtm_input_check(in, nullptr, easu_con, flags)) != FSR1_OK) return rc;
   if (y1 == 0) y1 = out->height;
   if (y0 >= y1 || y1 > out->height) return FSR1_ERR_INVALID_ARGUMENT;
   if (!window_holds(out, (int)y0, (int)y1 - 1)) return FSR1_ERR_WINDOW;
@@ -419,7 +441,7 @@ int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_im
   e.y0 = (int)y0; e.y1 = (int)y1;
   if ((flags & FSR1_FLAG_FUSED) && !(flags & (FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_CLAMP | FSR1_FLAG_RCAS_DENOISE |
                                               FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA | FSR1_FLAG_OUTPUT_SQUARE))) {
-    const cudaError_t err = launch_fused_h_post(e, rcas_con[1], q, (int)out->format, s, &name);
+    const cudaError_t err = launch_fused_h_post(e, rcas_con[1], q, (int)out->format, s, &name, srtm_in);
     if (err == cudaSuccess) {
       t_last_kernel = name;
       g_launches.fetch_add(1);

@@ -246,14 +246,15 @@ bool halo_sync_consumed();
 cudaError_t launch_easu_direct(const EasuParams& p, int format, bool exact, cudaStream_t s, const char** name);
 cudaError_t launch_rcas_direct(const RcasParams& p, int format, bool exact, cudaStream_t s, const char** name);
 // Packed-half production kernels.  Return cudaErrorNotSupported when the image layout does not
-// meet their alignment needs (the caller then falls back to the direct kernels).
-cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name);
+// meet their alignment needs (the caller then falls back to the direct kernels).  srtm_in: FSR1_FLAG_SRTM_INPUT (the caller
+// must not fall back then: no other kernel applies it).
+cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in = false);
 cudaError_t launch_rcas_h_packed(const RcasParams& p, cudaStream_t s, const char** name);
 // UNORM images through the TMA-tiled 2x EASU / packed RCAS kernels: cudaErrorNotSupported when not applicable
 cudaError_t launch_easu_u_tiled(const EasuParams& p, int format, cudaStream_t s, const char** name);
 cudaError_t launch_rcas_u_packed(const RcasParams& p, int format, cudaStream_t s, const char** name);
 // EASU -> RCAS in one kernel (RGBA16F, exactly 2x, out-of-image taps read 0): e.in = input, e.out = final output, rows [e.y0, e.y1)
-cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name);
+cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in = false);
 cudaError_t launch_easu_f32_tiled(const EasuParams& p, cudaStream_t s, const char** name);  // RGBA32F, exactly 2x
 cudaError_t launch_easu_h_precise(const EasuParams& p, cudaStream_t s, const char** name);  // RGBA16F io, fp32 math, 2x
 cudaError_t launch_rcas_f32_packed(const RcasParams& p, cudaStream_t s, const char** name);

@@ -25,7 +25,13 @@
 //   easu_u_quad2x_kernel  the same for R8G8B8A8_UNORM images (4-byte texels, decode pass, fused re-encode).
 //   easu_h_pairs_kernel   any other scale >= 1; 64x32 output tile per CTA; lane = one output column and a VERTICAL
 //                         pixel pair.
+// kSrtmIn (FSR1_FLAG_SRTM_INPUT, RGBA16F kernels): phase 1 first replaces each box texel by FsrSrtmF of it, rounded to half
+// (srtm_texel, fsr1_post.cuh), and takes the luma from that half texel; the taps then read the transformed tile.  It runs after
+// clamp_fixup, on the raw texels the fixup copied, so each texel is transformed once.  Its generic-proxy stores into the TMA buffer
+// precede the barrier that closes the tile; the fence_proxy_async thread 0 issues before the next TMA load into that buffer orders
+// them, as it does the tap loop's reads.
 #include "fsr1_easu_quad.cuh"
+#include "fsr1_post.cuh"
 
 namespace fsr1 {
 
@@ -140,6 +146,7 @@ __host__ __device__ inline size_t pairs_smem_bytes(int BW, int BH) {
   return off + 16 + 128;  // + barriers + slack for the manual 128B alignment
 }
 
+template <bool kSrtmIn = false>
 __global__ void __launch_bounds__(kThreads, 3)
 easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap, const int BW, const int BH,
                     const int tiles_x, const int n_tiles) {
@@ -202,7 +209,11 @@ easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap
     __syncthreads();
   }
 
-  for (int i = tid; i < n; i += kThreads) L[i] = texel_luma(tile[i]);  // phase 1
+  for (int i = tid; i < n; i += kThreads) {  // phase 1
+    uint2 c = tile[i];
+    if (kSrtmIn) tile[i] = c = srtm_texel(c);
+    L[i] = texel_luma(c);
+  }
   __syncthreads();
 
   // phase 2 over the (BW-2)x(BH-2) inner texels, flattened so that all lanes stay busy
@@ -263,7 +274,7 @@ template <int NW> struct __align__(128) QuadSmem {
   uint64_t bar[2];
 };
 
-template <int NW, int MINB>
+template <int NW, int MINB, bool kSrtmIn = false>
 __global__ void __launch_bounds__(NW * 32, MINB)
 easu_h_quad2x_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap, const int tiles_x,
                      const int n_tiles, const int mbase) {
@@ -306,7 +317,11 @@ easu_h_quad2x_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tma
       fence_proxy_async();  // these generic-proxy writes are later overwritten by a TMA (async proxy) load
       __syncthreads();
     }
-    for (int i = tid; i < C::kElems; i += NT) sm.L[i] = texel_luma(tile[i]);
+    for (int i = tid; i < C::kElems; i += NT) {
+      uint2 c = tile[i];
+      if (kSrtmIn) tile[i] = c = srtm_texel(c);
+      sm.L[i] = texel_luma(c);
+    }
     __syncthreads();
     for (int idx = tid; idx < kQSW * C::kSH; idx += NT) {
       const int j = idx / kQSW, i = idx - j * kQSW;
@@ -476,7 +491,7 @@ cudaError_t launch_easu_u_tiled(const EasuParams& p, int format, cudaStream_t s,
   return cudaGetLastError();
 }
 
-cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name) {
+cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in) {
   // layout requirements of TMA and of the vector stores
   if ((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15) || (reinterpret_cast<uintptr_t>(p.out.base) & 15) ||
       (p.out.pitch & 15))
@@ -491,8 +506,13 @@ cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char*
     constexpr int NW = 4, CY = 2 * NW;
     if (!make_tmap(&tmap, p.in, kQBW, CY + 3)) return cudaErrorNotSupported;
     const QuadGrid g = quad_grid(p, CY, (p.sync.ready[0] || p.sync.ready[1]) ? 6 : 7);
-    easu_h_quad2x_kernel<NW, 7><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
-    *name = "easu_h_quad2x<4w,7/sm,tma2>";
+    if (srtm_in) {
+      easu_h_quad2x_kernel<NW, 7, true><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
+      *name = "easu_h_quad2x<4w,7/sm,tma2,srtm_in>";
+    } else {
+      easu_h_quad2x_kernel<NW, 7><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
+      *name = "easu_h_quad2x<4w,7/sm,tma2>";
+    }
     return cudaGetLastError();
   }
 
@@ -505,15 +525,21 @@ cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char*
   if (smem > 200 * 1024) return cudaErrorNotSupported;
   if (!make_tmap(&tmap, p.in, BW, BH)) return cudaErrorNotSupported;
   if (smem > 48 * 1024) {  // per device and cheap: set on every launch that needs the opt-in
-    cudaError_t e = cudaFuncSetAttribute(easu_h_pairs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = srtm_in ? cudaFuncSetAttribute(easu_h_pairs_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                            : cudaFuncSetAttribute(easu_h_pairs_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
   const int tiles_x = (p.out.w + kTileW - 1) / kTileW, n_tiles = tiles_x * ((p.y1 - p.y0 + kTileH - 1) / kTileH);
   int per_sm = 3;
   while (per_sm > 1 && (size_t)per_sm * (smem + 1024) > 220 * 1024) per_sm--;
   const int grid = n_tiles < per_sm * sm_count() ? n_tiles : per_sm * sm_count();
-  easu_h_pairs_kernel<<<grid, kThreads, smem, s>>>(p, tmap, BW, BH, tiles_x, n_tiles);
-  *name = "easu_h_vpairs<64x32,persistent,tma2>";
+  if (srtm_in) {
+    easu_h_pairs_kernel<true><<<grid, kThreads, smem, s>>>(p, tmap, BW, BH, tiles_x, n_tiles);
+    *name = "easu_h_vpairs<64x32,persistent,tma2,srtm_in>";
+  } else {
+    easu_h_pairs_kernel<false><<<grid, kThreads, smem, s>>>(p, tmap, BW, BH, tiles_x, n_tiles);
+    *name = "easu_h_vpairs<64x32,persistent,tma2>";
+  }
   return cudaGetLastError();
 }
 

@@ -25,6 +25,9 @@
 //   output rows o in [2 m0, 2 m0 + 2n - 1] ∩ [ya, yb): mid index o - 2 m0 + 1, needs indices -1/+1 around it.
 // Out-of-image mid pixels hold 0 (D3D12 Load semantics, ffx_fsr1.h:698-707 through FSR_Pass.hlsl:61); FSR1_FLAG_RCAS_CLAMP is not
 // implemented here (the caller falls back to the two-kernel path).
+// kSrtmIn (FSR1_FLAG_SRTM_INPUT): phase 1 of a step first replaces each texel it covers by FsrSrtmF of it, rounded to half, as
+// easu_h_quad2x_kernel does (fsr1_easu_tiled.cu: after clamp_fixup, luma from the half texel; the fence_proxy_async before the next
+// TMA load into the buffer orders the stores).  Those kFBW (n + 3) texels are exactly the ones the step's taps read.
 #include "fsr1_easu_quad.cuh"
 #include "fsr1_post.cuh"
 #include "fsr1_rcas_math.cuh"
@@ -215,7 +218,7 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
   }
 }
 
-template <int NW, typename SO>
+template <int NW, typename SO, bool kSrtmIn>
 __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMap& tmap, const PostParams* q) {
   using C = FusedCfg<NW>;
   constexpr int NT = NW * 32, CY = C::kCY;
@@ -257,7 +260,11 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
       __syncthreads();
     }
     // phases 1 and 2 on the rows this step needs (n + 3 texel rows, n + 1 rows of terms)
-    for (int i = tid; i < kFBW * (n + 3); i += NT) sm.L[i] = texel_luma(tile[i]);
+    for (int i = tid; i < kFBW * (n + 3); i += NT) {
+      uint2 c = tile[i];
+      if (kSrtmIn) tile[i] = c = srtm_texel(c);
+      sm.L[i] = texel_luma(c);
+    }
     __syncthreads();
     for (int idx = tid; idx < kFSW * (n + 1); idx += NT) {
       const int j = idx / kFSW, i = idx - j * kFSW;
@@ -285,17 +292,17 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
   halo_sync_end(p.sync);
 }
 
-template <int NW, int MINB>
+template <int NW, int MINB, bool kSrtmIn = false>
 __global__ void __launch_bounds__(NW * 32, MINB)
 fused_h_quad2x_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap) {
-  fused_body<NW, void>(p, tmap, nullptr);
+  fused_body<NW, void, kSrtmIn>(p, tmap, nullptr);
 }
 
 // fsr1_upscale_post: the same kernel with the display epilogue in RCAS's store (SO: __half, Unorm8, Unorm10)
-template <int NW, int MINB, typename SO>
+template <int NW, int MINB, typename SO, bool kSrtmIn = false>
 __global__ void __launch_bounds__(NW * 32, MINB)
 fused_h_quad2x_post_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap, const __grid_constant__ PostParams q) {
-  fused_body<NW, SO>(p, tmap, &q);
+  fused_body<NW, SO, kSrtmIn>(p, tmap, &q);
 }
 
 #ifndef FSR1_CPU_EMU
@@ -331,7 +338,7 @@ static cudaError_t fused_setup(const EasuParams& e, uint32_t sharp_h2, int out_a
   return cudaSuccess;
 }
 
-cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name) {
+cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in) {
   if (clamp) return cudaErrorNotSupported;
   CUtensorMap tmap;
   FusedParams p;
@@ -339,8 +346,13 @@ cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cu
   long long grid = 0;
   const cudaError_t err = fused_setup(e, sharp_h2, 16, tmap, p, per_sm, grid);
   if (err != cudaSuccess) return err;
-  fused_h_quad2x_kernel<4, 7><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
-  *name = per_sm == 7 ? "fused_easu_rcas_h_quad2x<4w,7/sm,tma2,strips>" : "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips>";
+  if (srtm_in) {
+    fused_h_quad2x_kernel<4, 7, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
+    *name = per_sm == 7 ? "fused_easu_rcas_h_quad2x<4w,7/sm,tma2,strips,srtm_in>" : "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,srtm_in>";
+  } else {
+    fused_h_quad2x_kernel<4, 7><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
+    *name = per_sm == 7 ? "fused_easu_rcas_h_quad2x<4w,7/sm,tma2,strips>" : "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips>";
+  }
   return cudaGetLastError();
 }
 
@@ -348,25 +360,37 @@ cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cu
 constexpr int kPostPerSm = 6;
 
 cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const PostParams& q, int out_format, cudaStream_t s,
-                                const char** name) {
+                                const char** name, bool srtm_in) {
   CUtensorMap tmap;
   FusedParams p;
   int per_sm = kPostPerSm;
   long long grid = 0;
   const cudaError_t err = fused_setup(e, sharp_h2, out_format == 1 ? 16 : 8, tmap, p, per_sm, grid);
   if (err != cudaSuccess) return err;
-  switch (out_format) {
-    case 1:
+  switch (out_format * 2 + (srtm_in ? 1 : 0)) {
+    case 2:
       fused_h_quad2x_post_kernel<4, kPostPerSm, __half><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
       *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f>";
       break;
-    case 3:
+    case 6:
       fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm8><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
       *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8>";
       break;
-    case 4:
+    case 8:
       fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm10><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
       *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2>";
+      break;
+    case 3:
+      fused_h_quad2x_post_kernel<4, kPostPerSm, __half, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f,srtm_in>";
+      break;
+    case 7:
+      fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm8, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8,srtm_in>";
+      break;
+    case 9:
+      fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm10, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2,srtm_in>";
       break;
     default: return cudaErrorNotSupported;
   }

@@ -99,6 +99,16 @@ __device__ __forceinline__ float4 apply_op(int op, float4 c, const ImgView& aux,
   }
 }
 
+// ---- FSR1_FLAG_SRTM_INPUT: FsrSrtmF as the EASU kernels load each texel ------------------------------------------------------------
+// One RGBA16F texel -> fp32 -> FsrSrtmF -> rounded once to half: the texel fsr1_srtm(in, I, 0) writes into an RGBA16F image I.
+__device__ __forceinline__ uint2 srtm_texel(uint2 t) {
+  const float2 rg = __half22float2(*reinterpret_cast<const __half2*>(&t.x));
+  const float2 ba = __half22float2(*reinterpret_cast<const __half2*>(&t.y));
+  const float4 c = apply_op(kOpSrtm, make_float4(rg.x, rg.y, ba.x, ba.y), ImgView{}, 0, 0.0f, 0u, 0, 0, 0, 0);
+  const __half2 o0 = __floats2half2_rn(c.x, c.y), o1 = __floats2half2_rn(c.z, c.w);
+  return make_uint2(*reinterpret_cast<const uint32_t*>(&o0), *reinterpret_cast<const uint32_t*>(&o1));
+}
+
 // ---- the display epilogue of fsr1_upscale_post ---------------------------------------------------------------------------
 // ops bits: FSR1_POST_* of include/fsr1_b200.h, applied in this order
 enum { kPostSrtmInv = 1, kPostLfga = 2, kPostTepd8 = 4, kPostTepd10 = 8 };
@@ -209,7 +219,7 @@ __device__ __forceinline__ void post_pair(const PostParams& q, const PostCursor&
 // launchers (fsr1_fused.cu, fsr1_rcas_packed.cu); out_format 1 RGBA16F, 3 RGBA8_UNORM, 4 RGB10A2_UNORM.  cudaErrorNotSupported: the
 // frame or layout is not one the kernel takes (nothing launched).
 cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const PostParams& q, int out_format, cudaStream_t s,
-                                const char** name);
+                                const char** name, bool srtm_in = false);
 cudaError_t launch_rcas_h_post(const RcasParams& p, const PostParams& q, int out_format, cudaStream_t s, const char** name);
 
 }  // namespace fsr1

@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post */
+#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT */
 
 enum {
   FSR1_OK = 0,
@@ -85,6 +85,18 @@ enum {
                                        half2 structure-of-arrays registers, every operation a packed half operation with its own
                                        rounding.  Bit-identical to FSR1_FLAG_H_REFERENCE (the reference's Hx2 and H sources agree
                                        bit for bit); honours RCAS_CLAMP, RCAS_DENOISE, RCAS_PASSTHROUGH_ALPHA.  A parity path. */
+  FSR1_FLAG_SRTM_INPUT = 1u << 11,  /* the input holds LINEAR HDR values: EASU reads FsrSrtmF(texel) (ffx_fsr1.h:1030-1046, the tonemap
+                                       before the filter) for every input texel, applied as the kernel loads it, so the caller's input is
+                                       never written and no extra pass runs.  On rows [y0, y1) the result is bit-identical to the
+                                       flag-free call on the RGBA16F image I = fsr1_srtm(in, I, 0, ...) over the same window (each texel:
+                                       half -> fp32 FsrSrtmF -> rounded once to half; EASU's luma comes from that half texel).  Undo it
+                                       after RCAS with fsr1_upscale_post's FSR1_POST_SRTM_INVERSE: the full HDR round trip.
+                                       fsr1_easu, fsr1_upscale*, fsr1_context_* and fsr1_shard_* take it (RCAS never sees it; the shard's
+                                       halo carries raw input rows and fsr1_easu_input_rows is unchanged: SRTM is pointwise).  RGBA16F
+                                       input on the TMA-tiled kernels only: FSR1_ERR_UNSUPPORTED, with nothing launched, for another input
+                                       format, EXACT / FORCE_DIRECT / H_REFERENCE / PRECISE, an input (or EASU output) whose base or pitch
+                                       is not 16-byte aligned, or constants that do not upscale (0 < con0.x, con0.y <= 1).
+                                       fsr1_rcas: FSR1_ERR_INVALID_ARGUMENT. */
   FSR1_FLAG_H_REFERENCE = 1u << 4   /* fp16 images only: the literal FsrEasuH / FsrRcasH arithmetic (packed-half
                                        algorithm, half magic numbers, per-operation half rounding), bit-identical
                                        to the reference's H source; a parity path, slower and LESS accurate than
