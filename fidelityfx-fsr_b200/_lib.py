@@ -13,6 +13,7 @@ FLAG_RCAS_DENOISE, FLAG_RCAS_PASSTHROUGH_ALPHA, FLAG_OUTPUT_SQUARE, FLAG_FUSED, 
 FLAG_SRTM_INPUT = 2048
 POST_SRTM_INVERSE, POST_LFGA, POST_TEPD8, POST_TEPD10 = 1, 2, 4, 8
 SHARD_ONE_STREAM, SHARD_SKIP_HALO, SHARD_TRACE, SHARD_HANDLE_BYTES = 1 << 16, 1 << 17, 1 << 18, 64
+SHARD_DYNAMIC = 1 << 19
 
 # every symbol include/fsr1_b200.h declares
 SYMBOLS = ["fsr1_easu", "fsr1_rcas", "fsr1_easu_input_rows", "fsr1_upscale", "fsr1_upscale_post", "fsr1_context_create",
@@ -22,7 +23,7 @@ SYMBOLS = ["fsr1_easu", "fsr1_rcas", "fsr1_easu_input_rows", "fsr1_upscale", "fs
            "fsr1_srtm_h", "fsr1_lfga_h", "fsr1_tepd_h",
            "fsr1_shard_create", "fsr1_shard_destroy", "fsr1_shard_geometry", "fsr1_shard_export", "fsr1_shard_attach",
            "fsr1_shard_attach_local", "fsr1_shard_input", "fsr1_shard_window", "fsr1_shard_output", "fsr1_shard_arena",
-           "fsr1_shard_submit", "fsr1_shard_wait", "fsr1_shard_status", "fsr1_shard_trace"]
+           "fsr1_shard_frame", "fsr1_shard_submit", "fsr1_shard_wait", "fsr1_shard_status", "fsr1_shard_trace"]
 
 
 class Image(ctypes.Structure):
@@ -99,6 +100,7 @@ def lib():
         fn.argtypes = [vp, u32, imgp]
     L.fsr1_shard_arena.argtypes = [vp]
     L.fsr1_shard_arena.restype = vp
+    L.fsr1_shard_frame.argtypes = [vp, u32, u32, u32, f32]
     L.fsr1_shard_submit.argtypes = [vp, u32, vp]
     L.fsr1_shard_wait.argtypes = [vp, u32, vp]
     L.fsr1_shard_status.argtypes = [vp]

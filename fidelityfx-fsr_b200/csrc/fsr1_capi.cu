@@ -231,6 +231,9 @@ int fsr1_easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16
   const bool exact = (flags & FSR1_FLAG_EXACT) != 0;
   cudaError_t e = cudaErrorNotSupported;
   const char* name = "";
+  // Which kernel runs may depend on the constants only through "exactly 2x" and "upscaling" (is_2x and the upscaling-only checks
+  // in the launchers): a dynamic fsr1_shard loads the kernels of each such kind of frame at create (frame_kind, fsr1_shard.cu).
+  // A new scale-dependent choice must become a kind there too.
   if (flags & FSR1_FLAG_H_REFERENCE) {
     if (in->format != FSR1_FORMAT_RGBA16F || exact) return FSR1_ERR_UNSUPPORTED;
     e = launch_easu_href(p, s, &name);

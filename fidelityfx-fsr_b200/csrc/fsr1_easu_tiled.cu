@@ -462,6 +462,8 @@ static int max_footprint(int n_out, int first, int tile, float scale, float offs
   return best;
 }
 
+// The scale tests of the launchers (this one, "upscaling only", and fused_setup's) are the kinds of frame a dynamic fsr1_shard
+// loads kernels for at create (frame_kind, fsr1_shard.cu): keep the two in step.
 static bool is_2x(const EasuParams& p) { return p.c0x == 0.5f && p.c0y == 0.5f && p.c0z == -0.25f && p.c0w == -0.25f; }
 
 // tiles of the 2x kernels: cells k in [-1, k_last], rows of cells from the one holding output row y0

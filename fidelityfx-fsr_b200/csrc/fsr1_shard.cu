@@ -19,8 +19,32 @@
 // Flow control is by sequence numbers in device memory, so it is independent of host timing on either side: a push
 // for the q-th use of a slot waits for credit q-1, EASU of use q waits for ready q.  Every spin is bounded (a wall
 // clock timeout sets an error word instead of hanging the GPU).
+//
+// Dynamic resolution (FSR1_SHARD_DYNAMIC, fsr1_shard_frame): every use of a slot may have its own render size rw x rh (the
+// top-left of the input resource) and sharpness.  The frame's plan — owned / needed / window rows, the rows pushed to each
+// neighbour and where they land in the neighbour's window — is a pure function of (rh, constants, world, rank), so both ends
+// of a push compute the same destination rows without talking.  Each slot's window has room for the tallest window of any
+// render height the shard accepts, on every rank (the arena layout is rank-independent).
+// The protocol, and the credit sent by the EASU (or fused) kernel's last CTA, are those of a static shard.  Two kernels read my
+// window during use q-1 of a slot: my EASU kernel, and my push, which copies my edge rows to BOTH neighbours in one launch and may
+// still wait for one neighbour's credit after my EASU has finished and credited the other.  The credit covers the EASU's reads.
+// My push's reads for use q-1 on the side of a neighbour are ordered before that neighbour's push for use q: they published the
+// neighbour's ready q-1, which its EASU of use q-1 waited for, and the neighbour writes its rows for use q (and submits) only after
+// its fsr1_shard_wait of use q-1.  Nothing orders them before the OTHER neighbour's push for use q, so that one must never write a
+// row my push reads for use q-1 on the opposite side.  With one height for every use that always holds (neighbours write halo
+// rows, my push reads owned rows).  With a height per use it does not by itself: at 8 ranks, a 100-row frame and then a 21-row
+// one put rank 2's rows for the second frame on window rows rank 1's push up reads for the first.  So fsr1_shard_create marks,
+// per rank, the window offsets the push to each side reads and the neighbour on each side writes, over the accepted heights from
+// in_h downwards, and stops at the first height at which a row written from below would be a row read by the push up of some
+// accepted height, or the mirror case (mark_push_rows); fsr1_shard_frame refuses every height below (FSR1_ERR_UNSUPPORTED).  In
+// practice that is heights of a few rows per rank.  With that, the neighbour's push for use q waits for my credit q-1, so it never
+// overwrites a row my EASU of use q-1 still reads, and it never writes a row my push of use q-1 may still read; my own rows for use q are
+// written after fsr1_shard_wait of use q-1 (which follows my push); and every row EASU reads for use q (needed rows, all inside
+// [owned(k-1).a, owned(k+1).b)) is written for use q, by me or by a neighbour, before ready q is released, so rows a previous frame
+// left in the window are never read.
 #include <new>
 #include <string.h>
+#include <vector>
 
 #include "../../include/fsr1_b200.h"
 #include "fsr1_common.cuh"
@@ -114,22 +138,43 @@ int bpp_of(uint32_t fmt) {
 
 struct Rows { uint32_t a, b; };  // [a, b)
 
+// the fsr1_shard_* bits of the create flags; the rest are FSR1_FLAG_* for the kernels
+constexpr uint32_t kShardFlags = FSR1_SHARD_ONE_STREAM | FSR1_SHARD_SKIP_HALO | FSR1_SHARD_TRACE | FSR1_SHARD_DYNAMIC;
+
+// Kinds of frame that fsr1_upscale may run on different kernels: exactly 2x (the fused / 2x-tiled kernels), any other upscale
+// (the any-scale tiled kernels), and everything else (direct kernels).  Whether the EASU kernel carries the halo hand-shake
+// itself is a property of the kind: RGBA16F upscales (2x and any scale) take launch_easu_h_tiled / the fused kernel, which do;
+// RGBA16F downscales, FSR1_FLAG_PRECISE, fp32 and UNORM frames take kernels that do not.  The kinds mirror the dispatch rules of
+// fsr1_upscale / fsr1_easu (is_2x and "upscaling only" in the launchers): a launcher that chose between kernels WITHIN a kind
+// would have to become a kind of its own here, or its second kernel would be loaded lazily while flag-waiting kernels spin.
+enum { kFrame2x = 0, kFrameUp = 1, kFrameOther = 2, kFrameKinds = 3 };
+
+// One use of a slot: render size, constants, and this rank's rows for it (fsr1_shard_frame; the create-time frame otherwise).
+struct FramePlan {
+  uint32_t rw, rh;
+  uint32_t econ[16], rcon[4];
+  Rows owned, needed, window;
+  Rows send[2];           // my rows the neighbour needs
+  uint32_t peer_win0[2];  // first logical row of the neighbour's window
+  int kind;               // kFrame*
+};
+
 }  // namespace
 
 struct fsr1_shard {
   uint32_t in_w, in_h, out_w, out_h, format, world, rank, slots, flags;
   int device;
-  uint32_t econ[16], rcon[4];
-  // geometry of THIS rank
-  Rows out_rows, easu_rows, owned, needed, window;
+  // geometry of THIS rank: the output slab is fixed, the input rows are per frame
+  Rows out_rows, easu_rows;
+  FramePlan base;              // the create-time frame: whole resource, create sharpness (fsr1_shard_geometry)
+  FramePlan plan[kMaxSlots];   // the next use of each slot
   // arena: [flags page][slot 0 window][slot 1 window]...; identical layout on every rank
   uint64_t pitch, slot_stride, arena_bytes;
   uint32_t win_rows_max;
+  uint32_t min_rh;             // FSR1_SHARD_DYNAMIC: the smallest render height accepted (see the header)
   unsigned char* arena;
   unsigned char* peer[2];      // [kFromUp] = arena of rank-1, [kFromDown] = arena of rank+1 (mapped), nullptr = none
   bool peer_is_ipc[2];
-  uint32_t peer_win0[2];       // first logical row of the neighbour's window
-  Rows send[2];                // my rows the neighbour needs
   unsigned char* tmp;          // slots x rows easu_rows; null when the frames take the fused kernel (no intermediate)
   unsigned char* out;          // slots x rows out_rows
   uint64_t out_pitch, tmp_slot_stride, out_slot_stride;
@@ -139,7 +184,8 @@ struct fsr1_shard {
   bool attached;
   unsigned long long* trace;  // FSR1_SHARD_TRACE: kTraceFrames x kTraceWords globaltimer stamps (device memory), else null
   unsigned long long frames;  // frames submitted
-  bool inkernel_sync;  // the EASU / fused kernel of this configuration carries the hand-shake itself (HaloSync)
+  bool kind_ok[kFrameKinds];        // a dry frame of this kind ran at create (its kernels are loaded)
+  bool inkernel_sync[kFrameKinds];  // the EASU / fused kernel of this kind of frame carries the hand-shake itself (HaloSync)
 };
 
 namespace {
@@ -151,18 +197,93 @@ Rows plan_easu_rows(const fsr1_shard* s, uint32_t r) {
   const Rows o = plan_out_rows(s, r);
   return Rows{o.a == 0 ? 0 : o.a - 1, o.b >= s->out_h ? s->out_h : o.b + 1};
 }
-Rows plan_owned(const fsr1_shard* s, uint32_t r) {
-  return Rows{(uint32_t)((uint64_t)r * s->in_h / s->world), (uint32_t)((uint64_t)(r + 1) * s->in_h / s->world)};
+// input rows of a frame `rh` rows tall
+Rows plan_owned(const fsr1_shard* s, uint32_t rh, uint32_t r) {
+  return Rows{(uint32_t)((uint64_t)r * rh / s->world), (uint32_t)((uint64_t)(r + 1) * rh / s->world)};
 }
-Rows plan_needed(const fsr1_shard* s, uint32_t r) {
+Rows plan_needed(const fsr1_shard* s, const uint32_t econ[16], uint32_t rh, uint32_t r) {
   const Rows e = plan_easu_rows(s, r);
   uint32_t first = 0, last = 0;
-  fsr1_easu_input_rows(s->econ, s->in_h, e.a, e.b, &first, &last);
+  fsr1_easu_input_rows(econ, rh, e.a, e.b, &first, &last);
   return Rows{first, last + 1};
 }
-Rows plan_window(const fsr1_shard* s, uint32_t r) {
-  const Rows o = plan_owned(s, r), n = plan_needed(s, r);
+Rows plan_window(const fsr1_shard* s, const uint32_t econ[16], uint32_t rh, uint32_t r) {
+  const Rows o = plan_owned(s, rh, r), n = plan_needed(s, econ, rh, r);
   return Rows{o.a < n.a ? o.a : n.a, o.b > n.b ? o.b : n.b};
+}
+
+float word_as_float(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
+
+int frame_kind(const uint32_t econ[16]) {
+  const float sx = word_as_float(econ[0]), sy = word_as_float(econ[1]);
+  if (sx == 0.5f && sy == 0.5f && word_as_float(econ[2]) == -0.25f && word_as_float(econ[3]) == -0.25f) return kFrame2x;
+  return sx > 0.0f && sx <= 1.0f && sy > 0.0f && sy <= 1.0f ? kFrameUp : kFrameOther;
+}
+
+// The plan of frame rw x rh for this rank, with the constants context_run builds (FsrEasuCon(rw, rh, rw, rh, out_w, out_h),
+// FsrRcasCon(sharpness)).  FSR1_ERR_UNSUPPORTED when some rank's halo would have to come from beyond its direct neighbours
+// (true whenever a slab is taller than the halo).  *win_rows: the tallest window of any rank at this height.
+int make_plan(const fsr1_shard* s, uint32_t rw, uint32_t rh, float sharpness, FramePlan* p, uint32_t* win_rows) {
+  p->rw = rw;
+  p->rh = rh;
+  fsr1_easu_con(p->econ, (float)rw, (float)rh, (float)rw, (float)rh, (float)s->out_w, (float)s->out_h);
+  fsr1_rcas_con(p->rcon, sharpness);
+  p->kind = frame_kind(p->econ);
+  uint32_t wmax = 0;
+  for (uint32_t r = 0; r < s->world; r++) {
+    const Rows n = plan_needed(s, p->econ, rh, r), w = plan_window(s, p->econ, rh, r);
+    const uint32_t lo = r == 0 ? 0 : plan_owned(s, rh, r - 1).a, hi = r + 1 == s->world ? rh : plan_owned(s, rh, r + 1).b;
+    if (n.a < lo || n.b > hi) return FSR1_ERR_UNSUPPORTED;
+    if (w.b - w.a > wmax) wmax = w.b - w.a;
+  }
+  if (win_rows) *win_rows = wmax;
+  const uint32_t rank = s->rank;
+  p->owned = plan_owned(s, rh, rank);
+  p->needed = plan_needed(s, p->econ, rh, rank);
+  p->window = plan_window(s, p->econ, rh, rank);
+  for (int side = 0; side < 2; side++) {
+    p->send[side] = Rows{0, 0};
+    p->peer_win0[side] = 0;
+    const bool has = side == kFromUp ? rank > 0 : rank + 1 < s->world;
+    if (!has) continue;
+    const uint32_t peer = side == kFromUp ? rank - 1 : rank + 1;
+    const Rows pn = plan_needed(s, p->econ, rh, peer);
+    const uint32_t a = p->owned.a > pn.a ? p->owned.a : pn.a, b = p->owned.b < pn.b ? p->owned.b : pn.b;
+    if (b > a) p->send[side] = Rows{a, b};
+    p->peer_win0[side] = plan_window(s, p->econ, rh, peer).a;
+  }
+  return FSR1_OK;
+}
+
+// FSR1_SHARD_DYNAMIC: marks, per rank, the offsets into its window of the rows its push to each side reads and the rows the
+// neighbour on each side writes, for frames of height rh; false when a row the lower neighbour writes is one the push UP reads,
+// or a row the upper neighbour writes is one the push DOWN reads, for this or for a height marked before (see the header).
+bool mark_push_rows(const fsr1_shard* s, const uint32_t econ[16], uint32_t rh, std::vector<std::vector<uint8_t>>& marks) {
+  enum : uint8_t { kReadUp = 1, kReadDown = 2, kWriteFromUp = 4, kWriteFromDown = 8 };
+  for (uint32_t r = 0; r < s->world; r++) {
+    const Rows o = plan_owned(s, rh, r), n = plan_needed(s, econ, rh, r), w = plan_window(s, econ, rh, r);
+    std::vector<uint8_t>& m = marks[r];
+    if (m.size() < w.b - w.a) m.resize(w.b - w.a, 0);
+    auto mark = [&](uint32_t a, uint32_t b, uint8_t bit, uint8_t other) {  // rows [a, b)
+      for (uint32_t y = a; y < b; y++) {
+        if (m[y - w.a] & other) return false;
+        m[y - w.a] |= bit;
+      }
+      return true;
+    };
+    for (int side = 0; side < 2; side++) {
+      const bool has = side == kFromUp ? r > 0 : r + 1 < s->world;
+      if (!has) continue;
+      const uint32_t peer = side == kFromUp ? r - 1 : r + 1;
+      const Rows po = plan_owned(s, rh, peer), pn = plan_needed(s, econ, rh, peer);
+      const uint32_t sa = o.a > pn.a ? o.a : pn.a, sb = o.b < pn.b ? o.b : pn.b;  // my rows the neighbour needs
+      const uint32_t ra = po.a > n.a ? po.a : n.a, rb = po.b < n.b ? po.b : n.b;  // the neighbour's rows I need
+      const bool ok = side == kFromUp ? mark(sa, sb, kReadUp, kWriteFromDown) && mark(ra, rb, kWriteFromUp, kReadDown)
+                                      : mark(sa, sb, kReadDown, kWriteFromUp) && mark(ra, rb, kWriteFromDown, kReadUp);
+      if (!ok) return false;
+    }
+  }
+  return true;
 }
 
 int cuda_rc(cudaError_t e) { return e == cudaSuccess ? FSR1_OK : FSR1_ERR_CUDA; }
@@ -176,6 +297,34 @@ struct DeviceGuard {  // calls may come from a thread whose current device is an
   }
   ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
+
+fsr1_image make_img(void* data, uint64_t pitch, uint32_t w, uint32_t h, uint32_t row0, uint32_t rows, uint32_t fmt) {
+  fsr1_image im;
+  im.data = data; im.pitch_bytes = pitch; im.width = w; im.height = h; im.row0 = row0; im.rows = rows; im.format = fmt; im.reserved = 0;
+  return im;
+}
+unsigned char* window_of(const fsr1_shard* s, unsigned char* arena, uint32_t slot) { return arena + kFlagBytes + (uint64_t)slot * s->slot_stride; }
+fsr1_image tmp_of(const fsr1_shard* s, uint32_t slot) {
+  return make_img(s->tmp + (uint64_t)slot * s->tmp_slot_stride, s->out_pitch, s->out_w, s->out_h, s->easu_rows.a,
+                  s->easu_rows.b - s->easu_rows.a, s->format);
+}
+uint32_t kernel_flags(const fsr1_shard* s) { return (s->flags & ~kShardFlags) | FSR1_FLAG_FUSED; }
+
+// One dry frame `p` on the zero-filled slot 0 (no halo protocol), through the intermediate if there is one: loads the kernels
+// such a frame takes and tells whether they carry the halo hand-shake.  Leaves slot 0 described as `p`.
+int dry_frame(fsr1_shard* s, const FramePlan& p, bool* inkernel) {
+  s->plan[0] = p;
+  fsr1_image win, out, tmp;
+  fsr1_shard_window(s, 0, &win);
+  fsr1_shard_output(s, 0, &out);
+  if (s->tmp) tmp = tmp_of(s, 0);
+  const fsr1::HaloSync none = {};
+  fsr1::set_halo_sync(&none);
+  const int rc = fsr1_upscale(&win, s->tmp ? &tmp : nullptr, &out, p.econ, p.rcon, s->out_rows.a, s->out_rows.b, kernel_flags(s), s->s_easu);
+  *inkernel = fsr1::halo_sync_consumed();
+  fsr1::set_halo_sync(nullptr);
+  return rc;
+}
 
 }  // namespace
 
@@ -193,31 +342,38 @@ int fsr1_shard_create(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_
   s->in_w = in_w; s->in_h = in_h; s->out_w = out_w; s->out_h = out_h; s->format = format;
   s->world = world; s->rank = rank; s->slots = slots; s->flags = flags;
   if (cudaGetDevice(&s->device) != cudaSuccess) { delete s; return FSR1_ERR_NO_DEVICE; }
-  fsr1_easu_con(s->econ, (float)in_w, (float)in_h, (float)in_w, (float)in_h, (float)out_w, (float)out_h);
-  fsr1_rcas_con(s->rcon, sharpness_stops);
+  const bool dynamic = (flags & FSR1_SHARD_DYNAMIC) != 0;
   s->out_rows = plan_out_rows(s, rank);
   s->easu_rows = plan_easu_rows(s, rank);
-  s->owned = plan_owned(s, rank);
-  s->needed = plan_needed(s, rank);
-  s->window = plan_window(s, rank);
   // every rank's halo must come from its direct neighbours only (true whenever a slab is taller than the halo)
-  s->win_rows_max = 0;
-  for (uint32_t r = 0; r < world; r++) {
-    const Rows n = plan_needed(s, r), w = plan_window(s, r);
-    const uint32_t lo = r == 0 ? 0 : plan_owned(s, r - 1).a, hi = r + 1 == world ? in_h : plan_owned(s, r + 1).b;
-    if (n.a < lo || n.b > hi) { delete s; return FSR1_ERR_UNSUPPORTED; }
-    if (w.b - w.a > s->win_rows_max) s->win_rows_max = w.b - w.a;
+  if (make_plan(s, in_w, in_h, sharpness_stops, &s->base, &s->win_rows_max) != FSR1_OK) { delete s; return FSR1_ERR_UNSUPPORTED; }
+  // FSR1_SHARD_DYNAMIC: the render heights accepted are those from in_h down to the first height whose push rows would meet another
+  // accepted height's (mark_push_rows) that pass the same rule; the windows take the tallest of them.  All of it is a function of
+  // the shard's arguments only: the same on every rank.  The same scan finds one render size of each kind of frame for the dry
+  // frames below (the create-time frame first, for its own kind).
+  uint32_t rep_w[kFrameKinds] = {0, 0, 0}, rep_h[kFrameKinds] = {0, 0, 0};
+  s->min_rh = in_h;
+  if (dynamic) {
+    const uint32_t fit_w = in_w < out_w ? in_w : out_w;
+    const uint32_t cand_w[4] = {in_w, fit_w, fit_w - 1, out_w / 2};  // fit_w - 1, out_w / 2 may be 0: skipped
+    std::vector<std::vector<uint8_t>> marks(world);
+    for (uint32_t rh = in_h; rh >= world; rh--) {
+      FramePlan p;
+      uint32_t win_rows = 0;
+      if (make_plan(s, in_w, rh, sharpness_stops, &p, &win_rows) != FSR1_OK) continue;  // the rule depends on rh only
+      if (!mark_push_rows(s, p.econ, rh, marks)) break;
+      s->min_rh = rh;
+      if (win_rows > s->win_rows_max) s->win_rows_max = win_rows;
+      for (uint32_t rw : cand_w) {
+        if (rw == 0 || rw > in_w) continue;
+        uint32_t econ[16];
+        fsr1_easu_con(econ, (float)rw, (float)rh, (float)rw, (float)rh, (float)out_w, (float)out_h);
+        const int k = frame_kind(econ);
+        if (!rep_h[k]) { rep_w[k] = rw; rep_h[k] = rh; }
+      }
+    }
   }
-  for (int side = 0; side < 2; side++) {
-    const bool has = side == kFromUp ? rank > 0 : rank + 1 < world;
-    s->send[side] = Rows{0, 0};
-    if (!has) continue;
-    const uint32_t peer = side == kFromUp ? rank - 1 : rank + 1;
-    const Rows pn = plan_needed(s, peer);
-    const uint32_t a = s->owned.a > pn.a ? s->owned.a : pn.a, b = s->owned.b < pn.b ? s->owned.b : pn.b;
-    if (b > a) s->send[side] = Rows{a, b};
-    s->peer_win0[side] = plan_window(s, peer).a;
-  }
+  for (uint32_t i = 0; i < slots; i++) s->plan[i] = s->base;
   s->pitch = ((uint64_t)in_w * bpp + 127) & ~(uint64_t)127;
   s->slot_stride = ((uint64_t)s->win_rows_max * s->pitch + 255) & ~(uint64_t)255;
   s->arena_bytes = kFlagBytes + s->slot_stride * slots;
@@ -257,8 +413,8 @@ int fsr1_shard_create(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_
       return FSR1_ERR_CUDA;
     }
   }
-  // One dry frame on the zero-filled slot 0 (no halo protocol).  Every frame of the shard has this frame's format, scale, layout and
-  // options, so it decides for all of them:
+  // One dry frame on the zero-filled slot 0 (no halo protocol).  Every frame of a static shard has this frame's format, scale, layout
+  // and options, so it decides for all of them:
   //  - whether they take the fused EASU->RCAS kernel.  It is tried first, without an intermediate; only a configuration it does not
   //    cover (fsr1_upscale then needs `tmp`) gets the intermediate, 66 MB per slot at 1080p->4K RGBA16F, and runs the frame again
   //    through the two kernels;
@@ -266,28 +422,35 @@ int fsr1_shard_create(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_
   //  - and it loads every kernel a frame uses NOW.  CUDA loads kernels lazily, on first launch, and loading may synchronise the
   //    context: a first-use load issued while a flag-waiting kernel spins would wait for that kernel, which (several ranks in ONE
   //    process) may be waiting for work this very host thread has not submitted yet.
-  {
-    fsr1_image win, out;
-    fsr1_shard_window(s, 0, &win);
-    fsr1_shard_output(s, 0, &out);
-    const uint32_t kflags = (flags & ~(uint32_t)(FSR1_SHARD_ONE_STREAM | FSR1_SHARD_SKIP_HALO | FSR1_SHARD_TRACE)) | FSR1_FLAG_FUSED;
-    const fsr1::HaloSync none = {};
-    fsr1::set_halo_sync(&none);
-    int rc = fsr1_upscale(&win, nullptr, &out, s->econ, s->rcon, s->out_rows.a, s->out_rows.b, kflags, s->s_easu);
+  // A dynamic shard's frames differ in scale, so it allocates the intermediate up front (any frame that is not exactly 2x needs it;
+  // its size depends on the fixed output slab only) and runs one dry frame of every kind a frame can be: the create-time frame for
+  // its kind, a representative render size for each other kind.  A kind whose dry frame is refused with FSR1_ERR_UNSUPPORTED (the
+  // flags exclude it) is refused by fsr1_shard_frame as well.
+  bool inkernel = false;
+  if (!dynamic) {
+    int rc = dry_frame(s, s->base, &inkernel);
     if (rc != FSR1_OK) {
-      if ((e = cudaMalloc((void**)&s->tmp, s->tmp_slot_stride * slots)) != cudaSuccess) {
-        fsr1::set_halo_sync(nullptr);
-        fsr1_shard_destroy(s);
-        return FSR1_ERR_CUDA;
-      }
-      fsr1_image tmp0 = {s->tmp, s->out_pitch, s->out_w, s->out_h, s->easu_rows.a, s->easu_rows.b - s->easu_rows.a, s->format, 0};
-      fsr1::set_halo_sync(&none);
-      rc = fsr1_upscale(&win, &tmp0, &out, s->econ, s->rcon, s->out_rows.a, s->out_rows.b, kflags, s->s_easu);
+      if ((e = cudaMalloc((void**)&s->tmp, s->tmp_slot_stride * slots)) != cudaSuccess) { fsr1_shard_destroy(s); return FSR1_ERR_CUDA; }
+      rc = dry_frame(s, s->base, &inkernel);
     }
-    s->inkernel_sync = fsr1::halo_sync_consumed();
-    fsr1::set_halo_sync(nullptr);
     if (rc != FSR1_OK) { fsr1_shard_destroy(s); return rc; }
+    s->kind_ok[s->base.kind] = true;
+    s->inkernel_sync[s->base.kind] = inkernel;
+  } else {
+    if ((e = cudaMalloc((void**)&s->tmp, s->tmp_slot_stride * slots)) != cudaSuccess) { fsr1_shard_destroy(s); return FSR1_ERR_CUDA; }
+    for (int k = 0; k < kFrameKinds; k++) {
+      if (!rep_h[k]) continue;
+      FramePlan p;
+      if (k == s->base.kind) p = s->base;
+      else make_plan(s, rep_w[k], rep_h[k], sharpness_stops, &p, nullptr);  // passed the rule in the scan
+      const int rc = dry_frame(s, p, &inkernel);
+      if (rc == FSR1_ERR_UNSUPPORTED && k != s->base.kind) continue;
+      if (rc != FSR1_OK) { fsr1_shard_destroy(s); return rc; }
+      s->kind_ok[k] = true;
+      s->inkernel_sync[k] = inkernel;
+    }
   }
+  s->plan[0] = s->base;
   if ((e = cudaDeviceSynchronize()) != cudaSuccess) { fsr1_shard_destroy(s); return FSR1_ERR_CUDA; }  // flags are zero before anyone attaches
   s->attached = world == 1 || (flags & FSR1_SHARD_SKIP_HALO);
   *out_sh = s;
@@ -319,12 +482,13 @@ int fsr1_shard_geometry(const fsr1_shard* s, fsr1_shard_info* info) {
   if (!s || !info) return FSR1_ERR_INVALID_ARGUMENT;
   info->out_row0 = s->out_rows.a; info->out_row1 = s->out_rows.b;
   info->easu_row0 = s->easu_rows.a; info->easu_row1 = s->easu_rows.b;
-  info->owned_row0 = s->owned.a; info->owned_row1 = s->owned.b;
-  info->needed_row0 = s->needed.a; info->needed_row1 = s->needed.b;
-  info->window_row0 = s->window.a; info->window_row1 = s->window.b;
-  info->send_up_row0 = s->send[kFromUp].a; info->send_up_row1 = s->send[kFromUp].b;
-  info->send_down_row0 = s->send[kFromDown].a; info->send_down_row1 = s->send[kFromDown].b;
-  info->halo_recv_bytes = (uint64_t)((s->owned.a - s->window.a) + (s->window.b - s->owned.b)) * s->in_w * bpp_of(s->format);
+  const FramePlan& p = s->base;
+  info->owned_row0 = p.owned.a; info->owned_row1 = p.owned.b;
+  info->needed_row0 = p.needed.a; info->needed_row1 = p.needed.b;
+  info->window_row0 = p.window.a; info->window_row1 = p.window.b;
+  info->send_up_row0 = p.send[kFromUp].a; info->send_up_row1 = p.send[kFromUp].b;
+  info->send_down_row0 = p.send[kFromDown].a; info->send_down_row1 = p.send[kFromDown].b;
+  info->halo_recv_bytes = (uint64_t)((p.owned.a - p.window.a) + (p.window.b - p.owned.b)) * s->in_w * bpp_of(s->format);
   info->arena_bytes = s->arena_bytes;
   return FSR1_OK;
 }
@@ -386,23 +550,33 @@ int fsr1_shard_attach_local(fsr1_shard* s, fsr1_shard* up, fsr1_shard* down) {
   return attach_done(s);
 }
 
-static fsr1_image make_img(void* data, uint64_t pitch, uint32_t w, uint32_t h, uint32_t row0, uint32_t rows, uint32_t fmt) {
-  fsr1_image im;
-  im.data = data; im.pitch_bytes = pitch; im.width = w; im.height = h; im.row0 = row0; im.rows = rows; im.format = fmt; im.reserved = 0;
-  return im;
+int fsr1_shard_frame(fsr1_shard* s, uint32_t slot, uint32_t render_w, uint32_t render_h, float sharpness_stops) {
+  if (!s || !(s->flags & FSR1_SHARD_DYNAMIC) || slot >= s->slots) return FSR1_ERR_INVALID_ARGUMENT;
+  if (!render_w || !render_h || render_w > s->in_w || render_h > s->in_h || s->world > render_h) return FSR1_ERR_INVALID_ARGUMENT;
+  if (render_h < s->min_rh) return FSR1_ERR_UNSUPPORTED;  // a neighbour's halo rows could meet rows my push of another height reads
+  FramePlan p;
+  uint32_t win_rows = 0;
+  const int rc = make_plan(s, render_w, render_h, sharpness_stops, &p, &win_rows);
+  if (rc != FSR1_OK) return rc;
+  // a kind of frame whose dry frame the kernels refused at create (its kernels are not loaded), and a window beyond the capacity
+  // (cannot happen: create sized the windows over every accepted height)
+  if (!s->kind_ok[p.kind] || win_rows > s->win_rows_max) return FSR1_ERR_UNSUPPORTED;
+  s->plan[slot] = p;
+  return FSR1_OK;
 }
-static unsigned char* window_of(const fsr1_shard* s, unsigned char* arena, uint32_t slot) { return arena + kFlagBytes + (uint64_t)slot * s->slot_stride; }
 
 int fsr1_shard_input(const fsr1_shard* s, uint32_t slot, fsr1_image* owned) {
   if (!s || !owned || slot >= s->slots) return FSR1_ERR_INVALID_ARGUMENT;
-  *owned = make_img(window_of(s, s->arena, slot) + (uint64_t)(s->owned.a - s->window.a) * s->pitch, s->pitch, s->in_w, s->in_h, s->owned.a,
-                    s->owned.b - s->owned.a, s->format);
+  const FramePlan& p = s->plan[slot];
+  *owned = make_img(window_of(s, s->arena, slot) + (uint64_t)(p.owned.a - p.window.a) * s->pitch, s->pitch, p.rw, p.rh, p.owned.a,
+                    p.owned.b - p.owned.a, s->format);
   return FSR1_OK;
 }
 
 int fsr1_shard_window(const fsr1_shard* s, uint32_t slot, fsr1_image* window) {
   if (!s || !window || slot >= s->slots) return FSR1_ERR_INVALID_ARGUMENT;
-  *window = make_img(window_of(s, s->arena, slot), s->pitch, s->in_w, s->in_h, s->window.a, s->window.b - s->window.a, s->format);
+  const FramePlan& p = s->plan[slot];
+  *window = make_img(window_of(s, s->arena, slot), s->pitch, p.rw, p.rh, p.window.a, p.window.b - p.window.a, s->format);
   return FSR1_OK;
 }
 
@@ -427,16 +601,17 @@ int fsr1_shard_submit(fsr1_shard* s, uint32_t slot, void* stream) {
   if ((e = cudaEventRecord(s->ev_in[slot], caller)) != cudaSuccess) return cuda_rc(e);
   const bool skip_halo = (s->flags & FSR1_SHARD_SKIP_HALO) != 0;  // measurement only: what the frame costs without the exchange
   const bool up = s->rank > 0 && !skip_halo, down = s->rank + 1 < s->world && !skip_halo;
+  const FramePlan& p = s->plan[slot];  // this use of the slot: both ends of a push compute the same rows from it
   if (up || down) {
     PushSide ps[2];
     for (int side = 0; side < 2; side++) {
       ps[side] = PushSide{nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr};
       const bool has = side == kFromUp ? up : down;
       if (!has) continue;
-      const Rows r = s->send[side];
+      const Rows r = p.send[side];
       uint32_t* pf = reinterpret_cast<uint32_t*>(s->peer[side]);
-      ps[side].src = reinterpret_cast<const uint4*>(window_of(s, s->arena, slot) + (uint64_t)(r.a - s->window.a) * s->pitch);
-      ps[side].dst = reinterpret_cast<uint4*>(window_of(s, s->peer[side], slot) + (uint64_t)(r.a - s->peer_win0[side]) * s->pitch);
+      ps[side].src = reinterpret_cast<const uint4*>(window_of(s, s->arena, slot) + (uint64_t)(r.a - p.window.a) * s->pitch);
+      ps[side].dst = reinterpret_cast<uint4*>(window_of(s, s->peer[side], slot) + (uint64_t)(r.a - p.peer_win0[side]) * s->pitch);
       ps[side].n16 = (uint32_t)((uint64_t)(r.b - r.a) * s->pitch / 16);
       ps[side].credit = flags + credit_idx(slot, side);
       ps[side].parts_done = flags + push_cnt_idx(slot, side);
@@ -453,11 +628,9 @@ int fsr1_shard_submit(fsr1_shard* s, uint32_t slot, void* stream) {
   fsr1_shard_window(s, slot, &win);
   fsr1_shard_output(s, slot, &out);
   fsr1_image tmp;
-  if (s->tmp)
-    tmp = make_img(s->tmp + (uint64_t)slot * s->tmp_slot_stride, s->out_pitch, s->out_w, s->out_h, s->easu_rows.a,
-                   s->easu_rows.b - s->easu_rows.a, s->format);
-  // fused whenever the kernel covers the frame (fsr1_shard_create allocated no intermediate then), else EASU + RCAS through `tmp`
-  const uint32_t kflags = (s->flags & ~(uint32_t)(FSR1_SHARD_ONE_STREAM | FSR1_SHARD_SKIP_HALO | FSR1_SHARD_TRACE)) | FSR1_FLAG_FUSED;
+  if (s->tmp) tmp = tmp_of(s, slot);
+  // fused whenever the kernel covers the frame (a static shard allocated no intermediate then), else EASU + RCAS through `tmp`
+  const uint32_t kflags = kernel_flags(s);
   // The whole frame runs on ONE stream, consecutive frames on the two streams in turn: the tail of frame i overlaps the start of
   // frame i+1 (and with two kernels, RCAS of frame i (ALU / XU / HBM-bound) overlaps EASU of frame i+1 (FMA-pipe-bound)) without an
   // event between the kernels of a frame.
@@ -473,13 +646,13 @@ int fsr1_shard_submit(fsr1_shard* s, uint32_t slot, void* stream) {
   hs.status = flags + kStatusIdx;
   hs.trace = s->trace ? s->trace + (size_t)(s->frames % kTraceFrames) * kTraceWords : nullptr;
   hs.seq = q;
-  const bool shake = up || down, inkernel = shake && s->inkernel_sync;
+  const bool shake = up || down, inkernel = shake && s->inkernel_sync[p.kind];
   if (shake && !inkernel) {
     halo_wait_kernel<<<1, 32, 0, sk>>>(hs.ready[kFromUp], hs.ready[kFromDown], q, flags + kStatusIdx);
     if ((e = cudaGetLastError()) != cudaSuccess) return cuda_rc(e);
   }
   if (inkernel) fsr1::set_halo_sync(&hs);
-  int rc = fsr1_upscale(&win, s->tmp ? &tmp : nullptr, &out, s->econ, s->rcon, s->out_rows.a, s->out_rows.b, kflags, sk);
+  int rc = fsr1_upscale(&win, s->tmp ? &tmp : nullptr, &out, p.econ, p.rcon, s->out_rows.a, s->out_rows.b, kflags, sk);
   const bool took = inkernel && fsr1::halo_sync_consumed();
   fsr1::set_halo_sync(nullptr);
   if (rc != FSR1_OK) return rc;

@@ -159,13 +159,16 @@ class ShardedUpscaler:
     `owned` / `out` are slot 0's tensors; upscale() is the one-frame convenience over slot 0.
     halo="p2p" with world > 1 gathers the ranks' CUDA IPC handles through torch.distributed in the constructor (a collective:
     every rank constructs at the same point); attach=False skips that for ranks living in one process (attach_local).
+    dynamic=True (p2p only): in_w x in_h is the input resource, the largest render size; frame(slot, render_w, render_h) gives the
+    next use of a slot its own render size and sharpness (FSR1_SHARD_DYNAMIC, fsr1_shard_frame) before its rows are written.
     """
 
     def __init__(self, in_w, in_h, out_w, out_h, world, rank, sharpness=0.25, dtype=None, device=None, flags=0, slots=1,
-                 halo=None, one_stream=False, group=None, skip_halo=False, attach=True, trace=False):
+                 halo=None, one_stream=False, group=None, skip_halo=False, attach=True, trace=False, dynamic=False):
         import torch
         self.rank, self.world, self.slots = int(rank), int(world), int(slots)
         self.in_w, self.in_h, self.out_w, self.out_h = in_w, in_h, out_w, out_h
+        self.sharpness, self.dynamic = sharpness, bool(dynamic)
         self.econ = api.easu_con(in_w, in_h, in_w, in_h, out_w, out_h)
         self.rcon = api.rcas_con(sharpness)
         self.plan = SlabPlan(in_h, out_h, world, self.econ)
@@ -178,6 +181,8 @@ class ShardedUpscaler:
             halo = "p2p" if self.device.type == "cuda" else "nccl"
         if halo not in ("p2p", "nccl"):
             raise ValueError("halo must be 'p2p' or 'nccl'")
+        if self.dynamic and halo != "p2p":
+            raise ValueError("dynamic=True needs halo='p2p' (the per-frame plan lives in the C ABI's shard)")
         self.halo_mode = halo
         self._win0 = self.plan.window_rows(rank)[0]
         self._shard = None
@@ -196,7 +201,8 @@ class ShardedUpscaler:
         with torch.cuda.device(self.device):
             _lib.check(L.fsr1_shard_create(ctypes.byref(h), self.in_w, self.in_h, self.out_w, self.out_h, fmt, self.world, self.rank,
                                            self.slots, ctypes.c_float(sharpness),
-                                           self.flags | (_lib.SHARD_ONE_STREAM if one_stream else 0) | (_lib.SHARD_SKIP_HALO if skip_halo else 0) | (_lib.SHARD_TRACE if trace else 0)))
+                                           self.flags | (_lib.SHARD_ONE_STREAM if one_stream else 0) | (_lib.SHARD_SKIP_HALO if skip_halo else 0) | (_lib.SHARD_TRACE if trace else 0)
+                                           | (_lib.SHARD_DYNAMIC if self.dynamic else 0)))
         self._shard = h
         info = _lib.ShardInfo()
         _lib.check(L.fsr1_shard_geometry(h, ctypes.byref(info)))
@@ -287,6 +293,26 @@ class ShardedUpscaler:
                 api.image(self.windows[slot], height=self.in_h, row0=self._win0), api.image(self.tmps[slot], height=self.out_h, row0=e0),
                 api.image(self.outputs[slot], height=self.out_h, row0=y0), self.econ, self.rcon, y0=y0, y1=y1, flags=self.flags)
         self._prepared[slot].launch(stream)
+
+    def frame(self, slot, render_w, render_h, sharpness=None):
+        """dynamic=True: the next use of `slot` upscales the top-left render_w x render_h of the resource with `sharpness` (None: the
+        constructor's).  Call it before writing the frame's rows; returns input(slot), the rank's owned rows of that frame
+        ([rows, render_w, 4]).  Every rank describes the same use of a slot with the same arguments."""
+        if not self.dynamic:
+            raise ValueError("frame() needs a ShardedUpscaler constructed with dynamic=True")
+        L = _lib.lib()
+        sharp = self.sharpness if sharpness is None else sharpness
+        _lib.check(L.fsr1_shard_frame(self._shard, slot, render_w, render_h, ctypes.c_float(sharp)))
+        a, w = _lib.Image(), _lib.Image()
+        _lib.check(L.fsr1_shard_input(self._shard, slot, ctypes.byref(a)))
+        _lib.check(L.fsr1_shard_window(self._shard, slot, ctypes.byref(w)))
+        plan, r = SlabPlan(render_h, self.out_h, self.world, api.easu_con(render_w, render_h, render_w, render_h, self.out_w, self.out_h)), self.rank
+        assert (a.row0, a.row0 + a.rows) == plan.owned_in_rows(r) and (w.row0, w.row0 + w.rows) == plan.window_rows(r)
+        assert (a.width, a.height, w.width, w.height) == (render_w, render_h, render_w, render_h)
+        self.inputs[slot], self.windows[slot] = _tensor_of(a, self.device), _tensor_of(w, self.device)
+        if slot == 0:
+            self.owned, self.window = self.inputs[0], self.windows[0]
+        return self.inputs[slot]
 
     # ------------------------------------------------------------------------------------------ common
     def input(self, slot=0):

@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT */
+#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame */
 
 enum {
   FSR1_OK = 0,
@@ -180,6 +180,9 @@ typedef struct fsr1_shard fsr1_shard;
                                             streams, whole frames in turn, so RCAS of frame i overlaps EASU of frame i+1)                  */
 #define FSR1_SHARD_TRACE (1u << 18)      /* keep device timestamps of the last 256 frames (fsr1_shard_trace)                          */
 #define FSR1_SHARD_SKIP_HALO (1u << 17)  /* MEASUREMENT ONLY: no halo exchange (slab borders are wrong); times the frame without it */
+#define FSR1_SHARD_DYNAMIC (1u << 19)    /* dynamic resolution: in_width x in_height is the input RESOURCE, the largest render size a frame
+                                            may use; fsr1_shard_frame gives each use of a slot its own render size and sharpness (the
+                                            create-time sharpness_stops is the default).  Allocates the intermediate at create.     */
 
 typedef struct fsr1_shard_info {   /* logical row ranges [row0, row1) of this rank */
   uint32_t out_row0, out_row1;       /* output slab                                                 */
@@ -192,8 +195,10 @@ typedef struct fsr1_shard_info {   /* logical row ranges [row0, row1) of this ra
   uint64_t arena_bytes;
 } fsr1_shard_info;
 
-/* `flags`: FSR1_FLAG_* for the kernels, optionally FSR1_SHARD_ONE_STREAM.  FSR1_ERR_UNSUPPORTED when a slab is
- * shorter than the halo it must supply (the halo would come from beyond the direct neighbours). */
+/* `flags`: FSR1_FLAG_* for the kernels, optionally FSR1_SHARD_ONE_STREAM / _DYNAMIC.  FSR1_ERR_UNSUPPORTED when a slab is
+ * shorter than the halo it must supply (the halo would come from beyond the direct neighbours); with FSR1_SHARD_DYNAMIC this is
+ * checked for the whole resource here and for each frame's render height in fsr1_shard_frame.  fsr1_shard_geometry always
+ * describes the whole-resource frame. */
 int fsr1_shard_create(fsr1_shard** shard, uint32_t in_width, uint32_t in_height, uint32_t out_width, uint32_t out_height,
                       uint32_t format, uint32_t world, uint32_t rank, uint32_t slots, float sharpness_stops, uint32_t flags);
 void fsr1_shard_destroy(fsr1_shard* shard);
@@ -205,6 +210,20 @@ int fsr1_shard_input(const fsr1_shard* shard, uint32_t slot, fsr1_image* owned);
 int fsr1_shard_window(const fsr1_shard* shard, uint32_t slot, fsr1_image* window); /* owned rows + halo (read-only)     */
 int fsr1_shard_output(const fsr1_shard* shard, uint32_t slot, fsr1_image* out);    /* the rank's output slab            */
 void* fsr1_shard_arena(const fsr1_shard* shard);
+/* FSR1_SHARD_DYNAMIC: describe the next use of `slot` (call it before writing the frame's input rows).  The input is the top-left
+ * render_width x render_height of the resource, as in fsr1_context_upscale_render; the constants are
+ * FsrEasuCon(rw, rh, rw, rh, out_w, out_h) and FsrRcasCon(sharpness_stops).  Afterwards fsr1_shard_input / fsr1_shard_window
+ * describe that frame's rows (rank k owns input rows [k*rh/world, (k+1)*rh/world), logical width rw, the resource's pitch) and
+ * fsr1_shard_submit runs it; the output slab does not change.  A slot keeps its last description; the first is the whole resource
+ * at the create sharpness, so a dynamic shard that is never given one launches exactly what a static shard launches.  Every rank
+ * must describe the same use of a slot with the same arguments.  Host-only: no CUDA call, nothing allocated.
+ * FSR1_ERR_INVALID_ARGUMENT: a shard created without FSR1_SHARD_DYNAMIC, a bad slot, a zero render size, one larger than the
+ * resource, or world > render_height.  FSR1_ERR_UNSUPPORTED: at that render height a rank's halo would have to come from beyond its
+ * direct neighbours (the rule of fsr1_shard_create); a render height below the shard's minimum, a few rows per rank, where a
+ * neighbour's rows for one frame could land on window rows a rank's push of the previous frame in the slot still reads (26 rows at
+ * 8 ranks from a resource of half the output size); or the kernels refused a frame of its kind (2x / other upscale / downscale)
+ * with the create flags when fsr1_shard_create tried one. */
+int fsr1_shard_frame(fsr1_shard* shard, uint32_t slot, uint32_t render_width, uint32_t render_height, float sharpness_stops);
 /* Upscale the frame in `slot`: ordered after everything already on `stream`; returns without waiting. */
 int fsr1_shard_submit(fsr1_shard* shard, uint32_t slot, void* stream);
 /* Orders `stream` after the slot's result (and after this rank's halo rows have left: the input may be rewritten). */
