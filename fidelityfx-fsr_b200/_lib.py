@@ -23,7 +23,8 @@ SYMBOLS = ["fsr1_easu", "fsr1_rcas", "fsr1_easu_input_rows", "fsr1_upscale", "fs
            "fsr1_srtm_h", "fsr1_lfga_h", "fsr1_tepd_h",
            "fsr1_shard_create", "fsr1_shard_destroy", "fsr1_shard_geometry", "fsr1_shard_export", "fsr1_shard_attach",
            "fsr1_shard_attach_local", "fsr1_shard_input", "fsr1_shard_window", "fsr1_shard_output", "fsr1_shard_arena",
-           "fsr1_shard_frame", "fsr1_shard_submit", "fsr1_shard_wait", "fsr1_shard_status", "fsr1_shard_trace"]
+           "fsr1_shard_frame", "fsr1_shard_submit", "fsr1_shard_wait", "fsr1_shard_status", "fsr1_shard_trace",
+           "fsr1_shard_create_post", "fsr1_shard_post"]
 
 
 class Image(ctypes.Structure):
@@ -90,6 +91,8 @@ def lib():
     L.fsr1_lfga_h.argtypes = [imgp, imgp, imgp, f32, u32, u32, vp]
     L.fsr1_tepd_h.argtypes = [imgp, imgp, imgp, ctypes.c_int, u32, u32, u32, vp]
     L.fsr1_shard_create.argtypes = [ctypes.POINTER(vp), u32, u32, u32, u32, u32, u32, u32, u32, f32, u32]
+    L.fsr1_shard_create_post.argtypes = [ctypes.POINTER(vp), u32, u32, u32, u32, u32, u32, postp, u32, u32, u32, f32, u32]
+    L.fsr1_shard_post.argtypes = [vp, u32, postp]
     L.fsr1_shard_destroy.argtypes = [vp]
     L.fsr1_shard_destroy.restype = None
     L.fsr1_shard_geometry.argtypes = [vp, ctypes.POINTER(ShardInfo)]

@@ -383,20 +383,16 @@ int post_tile(const fsr1_image* im, bool used, ImgView& v, int& fmt) {
   fmt = (int)im->format;
   return FSR1_OK;
 }
-}  // namespace
 
-int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, const uint32_t easu_con[16],
-                      const uint32_t rcas_con[4], const fsr1_post* post, uint32_t y0, uint32_t y1, uint32_t flags, void* stream) {
-  if (!post || post->ops == 0) return fsr1_upscale(in, tmp, out, easu_con, rcas_con, y0, y1, flags, stream);
-  NvtxRange range("FSR1 upscale post");
+// the epilogue's parameters from a post description with ops != 0, under the rules that depend on the description, the formats and
+// the flags only (fsr1::post_rules)
+int post_params(const fsr1_post* post, uint32_t in_format, uint32_t out_format, uint32_t flags, PostParams& q) {
   const uint32_t ops = post->ops;
   if (ops & ~kAllPost) return FSR1_ERR_INVALID_ARGUMENT;
   if ((ops & FSR1_POST_TEPD8) && (ops & FSR1_POST_TEPD10)) return FSR1_ERR_INVALID_ARGUMENT;
   if ((ops & FSR1_POST_LFGA) && !post->grain) return FSR1_ERR_INVALID_ARGUMENT;
+  if (flags & ~kAllFlags) return FSR1_ERR_INVALID_ARGUMENT;
   int rc;
-  if ((rc = check_image(in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
-  if (!easu_con || !rcas_con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
-  PostParams q;
   const bool tepd = (ops & (FSR1_POST_TEPD8 | FSR1_POST_TEPD10)) != 0;
   if ((rc = post_tile(post->grain, (ops & FSR1_POST_LFGA) != 0, q.grain, q.grain_fmt)) != FSR1_OK) return rc;
   if ((rc = post_tile(post->dither, tepd, q.dither, q.dither_fmt)) != FSR1_OK) return rc;
@@ -405,12 +401,25 @@ int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_im
   q.amount = post->lfga_amount;
   q.frame = post->frame;
   // formats: RGBA16F in; RGBA16F out, or with TEPD the matching UNORM code values (the rule of fsr1_tepd)
-  if (in->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
+  if (in_format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
   const uint32_t unorm = (ops & FSR1_POST_TEPD8) ? FSR1_FORMAT_RGBA8_UNORM : (ops & FSR1_POST_TEPD10) ? FSR1_FORMAT_RGB10A2_UNORM : 0;
-  if (out->format != FSR1_FORMAT_RGBA16F && (!unorm || out->format != unorm)) return FSR1_ERR_UNSUPPORTED;
+  if (out_format != FSR1_FORMAT_RGBA16F && (!unorm || out_format != unorm)) return FSR1_ERR_UNSUPPORTED;
   // the half-arithmetic parity paths, fp32 EXACT/direct kernels and EASU-only frames keep the separate passes
   if (flags & (FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_RCAS_HX2 | FSR1_FLAG_NO_RCAS))
     return FSR1_ERR_UNSUPPORTED;
+  return FSR1_OK;
+}
+}  // namespace
+
+int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, const uint32_t easu_con[16],
+                      const uint32_t rcas_con[4], const fsr1_post* post, uint32_t y0, uint32_t y1, uint32_t flags, void* stream) {
+  if (!post || post->ops == 0) return fsr1_upscale(in, tmp, out, easu_con, rcas_con, y0, y1, flags, stream);
+  NvtxRange range("FSR1 upscale post");
+  int rc;
+  if ((rc = check_image(in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
+  if (!easu_con || !rcas_con) return FSR1_ERR_INVALID_ARGUMENT;
+  PostParams q;
+  if ((rc = post_params(post, in->format, out->format, flags, q)) != FSR1_OK) return rc;
   const bool srtm_in = (flags & FSR1_FLAG_SRTM_INPUT) != 0;
   if (srtm_in && (rc = srtm_input_check(in, nullptr, easu_con, flags)) != FSR1_OK) return rc;
   if (y1 == 0) y1 = out->height;
@@ -444,7 +453,9 @@ int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_im
   e.y0 = (int)y0; e.y1 = (int)y1;
   if ((flags & FSR1_FLAG_FUSED) && !(flags & (FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_CLAMP | FSR1_FLAG_RCAS_DENOISE |
                                               FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA | FSR1_FLAG_OUTPUT_SQUARE))) {
+    if (t_sync) e.sync = *t_sync;  // sharded frame: the neighbour hand-shake rides inside the kernel, as in fsr1_upscale
     const cudaError_t err = launch_fused_h_post(e, rcas_con[1], q, (int)out->format, s, &name, srtm_in);
+    if (err == cudaSuccess && t_sync) t_sync_used = true;
     if (err == cudaSuccess) {
       t_last_kernel = name;
       g_launches.fetch_add(1);
@@ -617,3 +628,11 @@ int fsr1_context_upscale_host(fsr1_context* c, const void* in_host, uint64_t in_
 }
 
 }  // extern "C"
+
+namespace fsr1 {
+int post_rules(const fsr1_post* post, uint32_t in_format, uint32_t out_format, uint32_t flags) {
+  if (!post) return FSR1_ERR_INVALID_ARGUMENT;
+  PostParams q;
+  return post_params(post, in_format, out_format, flags, q);
+}
+}  // namespace fsr1

@@ -5,6 +5,8 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+struct fsr1_post;  // include/fsr1_b200.h
+
 namespace fsr1 {
 
 // Device view of an fsr1_image (include/fsr1_b200.h): logical size w x h, storage holds rows
@@ -241,6 +243,9 @@ void set_last_detail(int v);  // fsr1_capi.cu: detail word reported by fsr1_last
 // kernel that was launched took it (the TMA-tiled fp16 kernels do; otherwise the shard falls back to its own tiny wait / signal kernels)
 void set_halo_sync(const HaloSync* hs);
 bool halo_sync_consumed();
+// fsr1_capi.cu -> fsr1_shard.cu: the rules fsr1_upscale_post applies to the post description (ops, tiles), the formats and the flags,
+// with the error it would return; no CUDA call.  The frame's images (sizes, windows, alignment) are checked by each launch.
+int post_rules(const ::fsr1_post* post, uint32_t in_format, uint32_t out_format, uint32_t flags);
 
 // launchers (defined in the .cu files, called from fsr1_capi.cu)
 cudaError_t launch_easu_direct(const EasuParams& p, int format, bool exact, cudaStream_t s, const char** name);

@@ -42,6 +42,10 @@
 // written after fsr1_shard_wait of use q-1 (which follows my push); and every row EASU reads for use q (needed rows, all inside
 // [owned(k-1).a, owned(k+1).b)) is written for use q, by me or by a neighbour, before ready q is released, so rows a previous frame
 // left in the window are never read.
+//
+// Display output (fsr1_shard_create_post, fsr1_shard_post): every frame is fsr1_upscale_post with the shard's ops and the slot's
+// description (frame, amount, tiles) instead of fsr1_upscale, so the slab is written once in the display format.  The fused post
+// kernel and the tiled EASU before the RCAS post kernel carry HaloSync like their plain forms; nothing else about the protocol changes.
 #include <new>
 #include <string.h>
 #include <vector>
@@ -159,10 +163,21 @@ struct FramePlan {
   int kind;               // kFrame*
 };
 
+// The display steps of one use of a slot (fsr1_shard_post; the create-time description otherwise): the fsr1_post minus its ops, which
+// are the shard's, with copies of the caller's tile descriptors (the tiles themselves stay the caller's).
+struct SlotPost {
+  float lfga_amount;
+  uint32_t frame;
+  fsr1_image grain, dither;
+  bool has_grain, has_dither;
+};
+
 }  // namespace
 
 struct fsr1_shard {
-  uint32_t in_w, in_h, out_w, out_h, format, world, rank, slots, flags;
+  uint32_t in_w, in_h, out_w, out_h, format, out_format, world, rank, slots, flags;
+  uint32_t post_ops;           // FSR1_POST_* of every frame (0: RGBA16F slabs in the input's format, fsr1_upscale)
+  SlotPost post[kMaxSlots];    // the next use of each slot
   int device;
   // geometry of THIS rank: the output slab is fixed, the input rows are per frame
   Rows out_rows, easu_rows;
@@ -176,8 +191,8 @@ struct fsr1_shard {
   unsigned char* peer[2];      // [kFromUp] = arena of rank-1, [kFromDown] = arena of rank+1 (mapped), nullptr = none
   bool peer_is_ipc[2];
   unsigned char* tmp;          // slots x rows easu_rows; null when the frames take the fused kernel (no intermediate)
-  unsigned char* out;          // slots x rows out_rows
-  uint64_t out_pitch, tmp_slot_stride, out_slot_stride;
+  unsigned char* out;          // slots x rows out_rows, in out_format
+  uint64_t out_pitch, tmp_pitch, tmp_slot_stride, out_slot_stride;
   uint32_t seq[kMaxSlots];
   cudaStream_t s_comm, s_easu, s_rcas;
   cudaEvent_t ev_in[kMaxSlots], ev_push[kMaxSlots], ev_rcas[kMaxSlots];
@@ -305,22 +320,41 @@ fsr1_image make_img(void* data, uint64_t pitch, uint32_t w, uint32_t h, uint32_t
 }
 unsigned char* window_of(const fsr1_shard* s, unsigned char* arena, uint32_t slot) { return arena + kFlagBytes + (uint64_t)slot * s->slot_stride; }
 fsr1_image tmp_of(const fsr1_shard* s, uint32_t slot) {
-  return make_img(s->tmp + (uint64_t)slot * s->tmp_slot_stride, s->out_pitch, s->out_w, s->out_h, s->easu_rows.a,
+  return make_img(s->tmp + (uint64_t)slot * s->tmp_slot_stride, s->tmp_pitch, s->out_w, s->out_h, s->easu_rows.a,
                   s->easu_rows.b - s->easu_rows.a, s->format);
 }
 uint32_t kernel_flags(const fsr1_shard* s) { return (s->flags & ~kShardFlags) | FSR1_FLAG_FUSED; }
+
+void set_slot_post(fsr1_shard* s, uint32_t slot, const fsr1_post* post) {
+  SlotPost& d = s->post[slot];
+  d.lfga_amount = post->lfga_amount;
+  d.frame = post->frame;
+  d.has_grain = (s->post_ops & FSR1_POST_LFGA) && post->grain;
+  d.has_dither = (s->post_ops & (FSR1_POST_TEPD8 | FSR1_POST_TEPD10)) && post->dither;
+  if (d.has_grain) d.grain = *post->grain;
+  if (d.has_dither) d.dither = *post->dither;
+}
+
+// The frame described by slot `slot` (its plan and post) on stream `st`: fsr1_upscale_post, which is fsr1_upscale without post ops.
+int launch_frame(fsr1_shard* s, uint32_t slot, cudaStream_t st) {
+  const FramePlan& p = s->plan[slot];
+  fsr1_image win, out, tmp;
+  fsr1_shard_window(s, slot, &win);
+  fsr1_shard_output(s, slot, &out);
+  if (s->tmp) tmp = tmp_of(s, slot);
+  const SlotPost& d = s->post[slot];
+  const fsr1_post post = {s->post_ops, d.lfga_amount, d.has_grain ? &d.grain : nullptr, d.has_dither ? &d.dither : nullptr, d.frame, 0};
+  return fsr1_upscale_post(&win, s->tmp ? &tmp : nullptr, &out, p.econ, p.rcon, s->post_ops ? &post : nullptr, s->out_rows.a,
+                           s->out_rows.b, kernel_flags(s), st);
+}
 
 // One dry frame `p` on the zero-filled slot 0 (no halo protocol), through the intermediate if there is one: loads the kernels
 // such a frame takes and tells whether they carry the halo hand-shake.  Leaves slot 0 described as `p`.
 int dry_frame(fsr1_shard* s, const FramePlan& p, bool* inkernel) {
   s->plan[0] = p;
-  fsr1_image win, out, tmp;
-  fsr1_shard_window(s, 0, &win);
-  fsr1_shard_output(s, 0, &out);
-  if (s->tmp) tmp = tmp_of(s, 0);
   const fsr1::HaloSync none = {};
   fsr1::set_halo_sync(&none);
-  const int rc = fsr1_upscale(&win, s->tmp ? &tmp : nullptr, &out, p.econ, p.rcon, s->out_rows.a, s->out_rows.b, kernel_flags(s), s->s_easu);
+  const int rc = launch_frame(s, 0, s->s_easu);
   *inkernel = fsr1::halo_sync_consumed();
   fsr1::set_halo_sync(nullptr);
   return rc;
@@ -332,15 +366,32 @@ extern "C" {
 
 int fsr1_shard_create(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_t out_w, uint32_t out_h, uint32_t format,
                       uint32_t world, uint32_t rank, uint32_t slots, float sharpness_stops, uint32_t flags) {
+  return fsr1_shard_create_post(out_sh, in_w, in_h, out_w, out_h, format, format, nullptr, world, rank, slots, sharpness_stops, flags);
+}
+
+int fsr1_shard_create_post(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_t out_w, uint32_t out_h, uint32_t format,
+                           uint32_t out_format, const fsr1_post* post, uint32_t world, uint32_t rank, uint32_t slots, float sharpness_stops,
+                           uint32_t flags) {
   if (!out_sh || !in_w || !in_h || !out_w || !out_h || !world || rank >= world || !slots || slots > kMaxSlots) return FSR1_ERR_INVALID_ARGUMENT;
-  const int bpp = bpp_of(format);
-  if (!bpp) return FSR1_ERR_INVALID_ARGUMENT;
+  const int bpp = bpp_of(format), out_bpp = bpp_of(out_format);
+  if (!bpp || !out_bpp) return FSR1_ERR_INVALID_ARGUMENT;
   if (world > in_h || world > out_h) return FSR1_ERR_INVALID_ARGUMENT;  // no empty slabs
+  // the display steps: fsr1_upscale_post's rules, before any CUDA call; without them the slabs are in the input's format
+  const uint32_t post_ops = post ? post->ops : 0u;
+  if (post_ops) {
+    const int rc = fsr1::post_rules(post, format, out_format, flags & ~kShardFlags);
+    if (rc != FSR1_OK) return rc;
+  } else if (out_format != format) {
+    return FSR1_ERR_UNSUPPORTED;
+  }
   fsr1_shard* s = new (std::nothrow) fsr1_shard();
   if (!s) return FSR1_ERR_INVALID_ARGUMENT;
   memset(s, 0, sizeof *s);
-  s->in_w = in_w; s->in_h = in_h; s->out_w = out_w; s->out_h = out_h; s->format = format;
+  s->in_w = in_w; s->in_h = in_h; s->out_w = out_w; s->out_h = out_h; s->format = format; s->out_format = out_format;
   s->world = world; s->rank = rank; s->slots = slots; s->flags = flags;
+  s->post_ops = post_ops;
+  if (post_ops)
+    for (uint32_t i = 0; i < slots; i++) set_slot_post(s, i, post);
   if (cudaGetDevice(&s->device) != cudaSuccess) { delete s; return FSR1_ERR_NO_DEVICE; }
   const bool dynamic = (flags & FSR1_SHARD_DYNAMIC) != 0;
   s->out_rows = plan_out_rows(s, rank);
@@ -377,8 +428,9 @@ int fsr1_shard_create(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_
   s->pitch = ((uint64_t)in_w * bpp + 127) & ~(uint64_t)127;
   s->slot_stride = ((uint64_t)s->win_rows_max * s->pitch + 255) & ~(uint64_t)255;
   s->arena_bytes = kFlagBytes + s->slot_stride * slots;
-  s->out_pitch = ((uint64_t)out_w * bpp + 127) & ~(uint64_t)127;
-  s->tmp_slot_stride = (uint64_t)(s->easu_rows.b - s->easu_rows.a) * s->out_pitch;
+  s->out_pitch = ((uint64_t)out_w * out_bpp + 127) & ~(uint64_t)127;
+  s->tmp_pitch = ((uint64_t)out_w * bpp + 127) & ~(uint64_t)127;  // the intermediate is in the input's format
+  s->tmp_slot_stride = (uint64_t)(s->easu_rows.b - s->easu_rows.a) * s->tmp_pitch;
   s->out_slot_stride = (uint64_t)(s->out_rows.b - s->out_rows.a) * s->out_pitch;
   cudaError_t e;
   int prio_lo = 0, prio_hi = 0;
@@ -426,6 +478,9 @@ int fsr1_shard_create(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_
   // its size depends on the fixed output slab only) and runs one dry frame of every kind a frame can be: the create-time frame for
   // its kind, a representative render size for each other kind.  A kind whose dry frame is refused with FSR1_ERR_UNSUPPORTED (the
   // flags exclude it) is refused by fsr1_shard_frame as well.
+  // With display steps every frame is fsr1_upscale_post with the shard's ops and output format, so the dry frames run it with the
+  // create-time description and load the post kernels (the fused post kernel, or tiled EASU + the RCAS post kernel; the srtm_in
+  // variants with FSR1_FLAG_SRTM_INPUT): which of them a frame takes depends on its kind, the flags and the output format only.
   bool inkernel = false;
   if (!dynamic) {
     int rc = dry_frame(s, s->base, &inkernel);
@@ -583,7 +638,15 @@ int fsr1_shard_window(const fsr1_shard* s, uint32_t slot, fsr1_image* window) {
 int fsr1_shard_output(const fsr1_shard* s, uint32_t slot, fsr1_image* out) {
   if (!s || !out || slot >= s->slots) return FSR1_ERR_INVALID_ARGUMENT;
   *out = make_img(s->out + (uint64_t)slot * s->out_slot_stride, s->out_pitch, s->out_w, s->out_h, s->out_rows.a, s->out_rows.b - s->out_rows.a,
-                  s->format);
+                  s->out_format);
+  return FSR1_OK;
+}
+
+int fsr1_shard_post(fsr1_shard* s, uint32_t slot, const fsr1_post* post) {
+  if (!s || slot >= s->slots || !post || !s->post_ops || post->ops != s->post_ops) return FSR1_ERR_INVALID_ARGUMENT;
+  const int rc = fsr1::post_rules(post, s->format, s->out_format, s->flags & ~kShardFlags);
+  if (rc != FSR1_OK) return rc;
+  set_slot_post(s, slot, post);
   return FSR1_OK;
 }
 
@@ -624,13 +687,7 @@ int fsr1_shard_submit(fsr1_shard* s, uint32_t slot, void* stream) {
     if ((e = cudaGetLastError()) != cudaSuccess) return cuda_rc(e);
     if ((e = cudaEventRecord(s->ev_push[slot], s->s_comm)) != cudaSuccess) return cuda_rc(e);
   }
-  fsr1_image win, out;
-  fsr1_shard_window(s, slot, &win);
-  fsr1_shard_output(s, slot, &out);
-  fsr1_image tmp;
-  if (s->tmp) tmp = tmp_of(s, slot);
   // fused whenever the kernel covers the frame (a static shard allocated no intermediate then), else EASU + RCAS through `tmp`
-  const uint32_t kflags = kernel_flags(s);
   // The whole frame runs on ONE stream, consecutive frames on the two streams in turn: the tail of frame i overlaps the start of
   // frame i+1 (and with two kernels, RCAS of frame i (ALU / XU / HBM-bound) overlaps EASU of frame i+1 (FMA-pipe-bound)) without an
   // event between the kernels of a frame.
@@ -652,7 +709,7 @@ int fsr1_shard_submit(fsr1_shard* s, uint32_t slot, void* stream) {
     if ((e = cudaGetLastError()) != cudaSuccess) return cuda_rc(e);
   }
   if (inkernel) fsr1::set_halo_sync(&hs);
-  int rc = fsr1_upscale(&win, s->tmp ? &tmp : nullptr, &out, p.econ, p.rcon, s->out_rows.a, s->out_rows.b, kflags, sk);
+  int rc = launch_frame(s, slot, sk);
   const bool took = inkernel && fsr1::halo_sync_consumed();
   fsr1::set_halo_sync(nullptr);
   if (rc != FSR1_OK) return rc;

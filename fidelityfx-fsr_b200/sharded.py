@@ -145,8 +145,10 @@ class _DevBuf:
 
 
 def _tensor_of(img, device):
-    """torch view [rows, width, 4] of an fsr1_image owned by the library."""
+    """torch view [rows, width, 4] of an fsr1_image owned by the library ([rows, width] int32 for RGB10A2_UNORM, as api.image takes)."""
     import torch
+    if img.format == _lib.FORMAT_RGB10A2_UNORM:
+        return torch.as_tensor(_DevBuf(img.data, (img.rows, img.width), (img.pitch_bytes, 4), "<i4"), device=device)
     es, typestr = {_lib.FORMAT_RGBA16F: (2, "<f2"), _lib.FORMAT_RGBA32F: (4, "<f4"), _lib.FORMAT_RGBA8_UNORM: (1, "|u1")}[img.format]
     return torch.as_tensor(_DevBuf(img.data, (img.rows, img.width, 4), (img.pitch_bytes, 4 * es, es), typestr), device=device)
 
@@ -161,14 +163,21 @@ class ShardedUpscaler:
     every rank constructs at the same point); attach=False skips that for ranks living in one process (attach_local).
     dynamic=True (p2p only): in_w x in_h is the input resource, the largest render size; frame(slot, render_w, render_h) gives the
     next use of a slot its own render size and sharpness (FSR1_SHARD_DYNAMIC, fsr1_shard_frame) before its rows are written.
+    srtm_inverse / grain, amount / tepd_bits, dither (p2p only): the display steps of api.upscale_post run inside every frame
+    (fsr1_shard_create_post), so output(slot) is the display image's rows: uint8 [rows, W, 4] with tepd_bits 8, int32 [rows, W] with 10,
+    float16 [rows, W, 4] otherwise.  post(slot, frame=...) describes the next use of a slot (fsr1_shard_post).  The grain / dither
+    tiles are device tensors the ranks read while frames are in flight; this object keeps a reference to the ones each slot uses.
     """
 
     def __init__(self, in_w, in_h, out_w, out_h, world, rank, sharpness=0.25, dtype=None, device=None, flags=0, slots=1,
-                 halo=None, one_stream=False, group=None, skip_halo=False, attach=True, trace=False, dynamic=False):
+                 halo=None, one_stream=False, group=None, skip_halo=False, attach=True, trace=False, dynamic=False,
+                 srtm_inverse=False, grain=None, amount=0.0, tepd_bits=0, dither=None):
         import torch
         self.rank, self.world, self.slots = int(rank), int(world), int(slots)
         self.in_w, self.in_h, self.out_w, self.out_h = in_w, in_h, out_w, out_h
         self.sharpness, self.dynamic = sharpness, bool(dynamic)
+        self._post_args = (bool(srtm_inverse), grain, amount, tepd_bits, dither)
+        self.has_post = bool(srtm_inverse) or grain is not None or tepd_bits != 0
         self.econ = api.easu_con(in_w, in_h, in_w, in_h, out_w, out_h)
         self.rcon = api.rcas_con(sharpness)
         self.plan = SlabPlan(in_h, out_h, world, self.econ)
@@ -183,6 +192,8 @@ class ShardedUpscaler:
             raise ValueError("halo must be 'p2p' or 'nccl'")
         if self.dynamic and halo != "p2p":
             raise ValueError("dynamic=True needs halo='p2p' (the per-frame plan lives in the C ABI's shard)")
+        if self.has_post and halo != "p2p":
+            raise ValueError("display steps (srtm_inverse, grain, tepd_bits) need halo='p2p' (they run inside the C ABI's shard)")
         self.halo_mode = halo
         self._win0 = self.plan.window_rows(rank)[0]
         self._shard = None
@@ -197,12 +208,18 @@ class ShardedUpscaler:
         import torch
         L = _lib.lib()
         fmt = {torch.float16: _lib.FORMAT_RGBA16F, torch.float32: _lib.FORMAT_RGBA32F, torch.uint8: _lib.FORMAT_RGBA8_UNORM}[dtype]
+        srtm_inverse, grain, amount, tepd_bits, dither = self._post_args
+        post, keep = api._post(srtm_inverse, grain, amount, tepd_bits, dither, 0)
+        out_fmt = {0: fmt, 8: _lib.FORMAT_RGBA8_UNORM, 10: _lib.FORMAT_RGB10A2_UNORM}[tepd_bits]
+        self._tiles = [(grain, dither)] * self.slots     # the tiles each slot's next use reads
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
-            _lib.check(L.fsr1_shard_create(ctypes.byref(h), self.in_w, self.in_h, self.out_w, self.out_h, fmt, self.world, self.rank,
-                                           self.slots, ctypes.c_float(sharpness),
-                                           self.flags | (_lib.SHARD_ONE_STREAM if one_stream else 0) | (_lib.SHARD_SKIP_HALO if skip_halo else 0) | (_lib.SHARD_TRACE if trace else 0)
-                                           | (_lib.SHARD_DYNAMIC if self.dynamic else 0)))
+            _lib.check(L.fsr1_shard_create_post(ctypes.byref(h), self.in_w, self.in_h, self.out_w, self.out_h, fmt, out_fmt,
+                                                ctypes.byref(post) if self.has_post else None, self.world, self.rank,
+                                                self.slots, ctypes.c_float(sharpness),
+                                                self.flags | (_lib.SHARD_ONE_STREAM if one_stream else 0) | (_lib.SHARD_SKIP_HALO if skip_halo else 0) | (_lib.SHARD_TRACE if trace else 0)
+                                                | (_lib.SHARD_DYNAMIC if self.dynamic else 0)))
+        del keep
         self._shard = h
         info = _lib.ShardInfo()
         _lib.check(L.fsr1_shard_geometry(h, ctypes.byref(info)))
@@ -313,6 +330,20 @@ class ShardedUpscaler:
         if slot == 0:
             self.owned, self.window = self.inputs[0], self.windows[0]
         return self.inputs[slot]
+
+    def post(self, slot, frame=0, amount=None, grain=None, dither=None):
+        """The display steps of the next use of `slot` (fsr1_shard_post): the TEPD `frame` of the positional dither, the LFGA amount and
+        the tiles; None keeps the constructor's amount / grain / dither.  The steps themselves (srtm_inverse, LFGA, tepd_bits) are the
+        constructor's."""
+        if not self.has_post:
+            raise ValueError("post() needs a ShardedUpscaler constructed with display steps (srtm_inverse, grain or tepd_bits)")
+        srtm_inverse, grain0, amount0, tepd_bits, dither0 = self._post_args
+        grain = grain0 if grain is None else grain
+        dither = dither0 if dither is None else dither
+        post, keep = api._post(srtm_inverse, grain, amount0 if amount is None else amount, tepd_bits, dither, frame)
+        _lib.check(_lib.lib().fsr1_shard_post(self._shard, slot, ctypes.byref(post)))
+        del keep
+        self._tiles[slot] = (grain, dither)
 
     # ------------------------------------------------------------------------------------------ common
     def input(self, slot=0):

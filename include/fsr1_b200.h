@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame */
+#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame, fsr1_shard_create_post / fsr1_shard_post */
 
 enum {
   FSR1_OK = 0,
@@ -299,6 +299,33 @@ int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_im
 int fsr1_context_upscale_post(fsr1_context* ctx, const void* in_dev, uint64_t in_pitch, uint32_t render_width,
                               uint32_t render_height, void* out_dev, uint64_t out_pitch, float sharpness_stops,
                               const fsr1_post* post, uint32_t flags, void* stream);
+
+/* Display output from the sharded frame stream: every frame of the shard is fsr1_upscale_post with `post` instead of fsr1_upscale,
+ * so each rank's output slab holds the display image's rows (for rows [out_row0, out_row1), bit-identical to the same rows of
+ * fsr1_upscale_post / fsr1_context_upscale_post on the whole frame) and no pass runs over the slabs afterwards.  fsr1_shard_create is
+ * fsr1_shard_create_post(..., format, format, NULL, ...).
+ *   format      the input's format; with post ops RGBA16F only.
+ *   out_format  the slabs' format: RGBA16F, or with TEPD the UNORM format it implies (RGBA8_UNORM for TEPD8, RGB10A2_UNORM for
+ *               TEPD10, 4 B/px); without post ops it must equal `format`.  fsr1_shard_output describes slabs in this format.
+ *   post        NULL or ops == 0: no display steps.  `post->ops` is fixed for the shard's life (it decides which kernels the create-time
+ *               dry frames load); the rest is the first description of every slot (fsr1_shard_post).  The tiles (grain, dither) are
+ *               whole device images on the rank's own device, read by every frame that uses them: the caller keeps them alive and
+ *               unchanged until those frames have completed (fsr1_shard_wait); the shard copies the descriptors, not the pixels.
+ * The rules are those of fsr1_upscale_post, all checked before any CUDA call: FSR1_ERR_INVALID_ARGUMENT for unknown ops bits, both TEPD
+ * bits, LFGA without a grain tile, a tile that is a window; FSR1_ERR_UNSUPPORTED for another input / output format, FSR1_FLAG_EXACT /
+ * FORCE_DIRECT / H_REFERENCE / RCAS_HX2 / NO_RCAS.  A static 2x shard whose frames take the fused post kernel allocates no intermediate;
+ * every other shard allocates an RGBA16F one, as fsr1_shard_create does.  The halo hand-shake rides inside the post kernels exactly as
+ * inside the plain ones (trace stamps [0]-[2]). */
+int fsr1_shard_create_post(fsr1_shard** shard, uint32_t in_width, uint32_t in_height, uint32_t out_width, uint32_t out_height,
+                           uint32_t format, uint32_t out_format, const fsr1_post* post, uint32_t world, uint32_t rank, uint32_t slots,
+                           float sharpness_stops, uint32_t flags);
+/* Describe the display steps of the next use of `slot`, as fsr1_shard_frame describes its render size: the TEPD `frame` of the
+ * positional dither FsrTepdDitF(pixel, frame), the LFGA amount and the grain / dither tiles.  `post->ops` must equal the shard's.  A slot
+ * keeps its last description; the first is the create-time `post`.  Host-only: no CUDA call, nothing allocated.
+ * FSR1_ERR_INVALID_ARGUMENT: a shard created without post ops, ops other than the shard's, a bad slot, or a description
+ * fsr1_upscale_post refuses (LFGA without a grain tile, a tile that is a window); FSR1_ERR_UNSUPPORTED: a grain tile that is not
+ * RGBA16F / RGBA32F.  The slot keeps its previous description on any error. */
+int fsr1_shard_post(fsr1_shard* shard, uint32_t slot, const fsr1_post* post);
 
 /* ---- constants through the ABI (for FFIs that cannot include fsr1_host.h) ---------------------- */
 void fsr1_easu_con(uint32_t con[16], float in_viewport_w, float in_viewport_h, float in_size_w, float in_size_h,
