@@ -16,7 +16,9 @@
 
 namespace fsr1 {
 
-__device__ __forceinline__ float texel_luma(uint2 t) {  // 2*luma = 0.5 B + (0.5 R + G); exact in fp32
+// 2*luma = 0.5 B + (0.5 R + G): two fp32 roundings, not exact (G = 2048 with R, B below 2^-12 rounds both), so the order of
+// the two FMAs is part of the result and every kernel that takes a luma from half texels must keep it
+__device__ __forceinline__ float texel_luma(uint2 t) {
   const float2 rg = __half22float2(u2h2(t.x));
   return fmaf(__low2float(u2h2(t.y)), 0.5f, fmaf(rg.x, 0.5f, rg.y));
 }

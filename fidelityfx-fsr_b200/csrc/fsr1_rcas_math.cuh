@@ -44,9 +44,13 @@ __device__ __forceinline__ __half2 luma2x(const Row3& c) {  // bL = bB*0.5 + (bR
   return __hfma2(c.b, kHalf, __hfma2(c.r, kHalf, c.g));
 }
 
-// packed APrxMedRcpH2 (ffx_a.h:1815): 16-bit magic subtract (no borrow for the arguments used here) + one Newton step
+// packed APrxMedRcpH2 (ffx_a.h:1815): 16-bit magic subtract + one Newton step.  The subtract wraps inside each 16-bit lane as the
+// reference's does: a 32-bit 0x778d778d - a would let a low lane above 0x778d (the denoise range of overflowing content: >= 30928,
+// inf or NaN) borrow from the other pixel's lane.  Per lane: (K | 0x8000) - (a & 0x7fff) cannot borrow across lanes, and the XOR
+// restores bit 15 of K - a.
 __device__ __forceinline__ __half2 prx_med_rcp_h2(__half2 a) {
-  const __half2 s = uh2(0x778d778du - hu2(a));
+  const uint32_t u = hu2(a);
+  const __half2 s = uh2((0xf78df78du - (u & 0x7fff7fffu)) ^ (~(u ^ 0x778d778du) & 0x80008000u));
   return __hmul2(s, __hfma2(__hneg2(s), a, __float2half2_rn(2.0f)));
 }
 

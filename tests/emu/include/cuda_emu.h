@@ -63,8 +63,9 @@ template <typename T> inline T __ldg(const T* p) { return *p; }
 struct __half { uint16_t b; };
 struct alignas(4) __half2 { __half x, y; };
 inline float h2f(__half h) { _Float16 v; memcpy(&v, &h.b, 2); return (float)v; }
-inline __half d2h(double d) { _Float16 v = (_Float16)d; __half h; memcpy(&h.b, &v, 2); return h; }  // one rounding (RNE)
-inline __half f2h(float f) { _Float16 v = (_Float16)f; __half h; memcpy(&h.b, &v, 2); return h; }
+// one rounding (RNE); a NaN result is the canonical 0x7fff the GPU's half arithmetic and conversions produce (the host's is 0xfe00)
+inline __half d2h(double d) { _Float16 v = (_Float16)d; __half h; memcpy(&h.b, &v, 2); if (d != d) h.b = 0x7fff; return h; }
+inline __half f2h(float f) { _Float16 v = (_Float16)f; __half h; memcpy(&h.b, &v, 2); if (f != f) h.b = 0x7fff; return h; }
 inline __half2 mkh2(__half a, __half b) { __half2 r; r.x = a; r.y = b; return r; }
 inline __half2 __floats2half2_rn(float a, float b) { return mkh2(f2h(a), f2h(b)); }
 inline __half2 __float2half2_rn(float a) { return mkh2(f2h(a), f2h(a)); }
@@ -89,8 +90,15 @@ inline __half2 __hmul2_rn(__half2 a, __half2 b) { return __hmul2(a, b); }
 inline __half2 __hmul2_sat(__half2 a, __half2 b) { return mkh2(f2h(__saturatef((float)((double)h2f(a.x) * h2f(b.x)))), f2h(__saturatef((float)((double)h2f(a.y) * h2f(b.y))))); }
 inline __half2 __hneg2(__half2 a) { a.x.b ^= 0x8000; a.y.b ^= 0x8000; return a; }
 inline __half2 __habs2(__half2 a) { a.x.b &= 0x7fff; a.y.b &= 0x7fff; return a; }
-inline __half hmin1(__half a, __half b) { return f2h(fminf(h2f(a), h2f(b))); }  // non-propagating, like HMNMX2
-inline __half hmax1(__half a, __half b) { return f2h(fmaxf(h2f(a), h2f(b))); }
+// non-propagating, like HMNMX2: a NaN operand yields the other one; -0 < +0 (fminf / fmaxf leave the sign of a zero result
+// unspecified, and glibc's depends on the operand order)
+inline bool hless1(__half a, __half b) {
+  const int ka = (a.b & 0x8000) ? -(int)(a.b & 0x7fff) - 1 : (int)a.b, kb = (b.b & 0x8000) ? -(int)(b.b & 0x7fff) - 1 : (int)b.b;
+  return ka < kb;
+}
+inline bool hnan1(__half a) { return (a.b & 0x7fff) > 0x7c00; }
+inline __half hmin1(__half a, __half b) { return hnan1(a) ? (hnan1(b) ? __half{0x7fff} : b) : hnan1(b) ? a : hless1(b, a) ? b : a; }
+inline __half hmax1(__half a, __half b) { return hnan1(a) ? (hnan1(b) ? __half{0x7fff} : b) : hnan1(b) ? a : hless1(a, b) ? b : a; }
 inline __half2 __hmin2(__half2 a, __half2 b) { return mkh2(hmin1(a.x, b.x), hmin1(a.y, b.y)); }
 inline __half2 __hmax2(__half2 a, __half2 b) { return mkh2(hmax1(a.x, b.x), hmax1(a.y, b.y)); }
 

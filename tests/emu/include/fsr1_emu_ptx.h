@@ -30,7 +30,9 @@ inline void tma_load_2d(void* dst, const CUtensorMap* map, int x, int y, uint64_
   emu_bar(bar)->fetch_add(1, std::memory_order_release);
 }
 inline void mbar_arrive(uint64_t* bar) { emu_bar(bar)->fetch_add(1, std::memory_order_release); }
-inline float rcp_approx(float a) { return 1.0f / a; }  // MUFU.RCP is within 1 ulp of this
+// MUFU.RCP is within 1 ulp of this, and that does not change a result: every caller passes a half and rounds the reciprocal to
+// half at once, and for every half x, 1/x lies at least 2 fp32 ulps from every half rounding boundary (tests/test_kernel_model.py)
+inline float rcp_approx(float a) { return 1.0f / a; }
 // min.s16x2
 inline uint32_t emu_min_s16x2(uint32_t a, uint32_t b) {
   const int16_t al = (int16_t)(a & 0xffff), ah = (int16_t)(a >> 16), bl = (int16_t)(b & 0xffff), bh = (int16_t)(b >> 16);
