@@ -8,6 +8,7 @@ LIB_PATH = os.path.join(HERE, "lib", "libfsr1_b200.so")
 
 FSR1_OK = 0
 FORMAT_RGBA16F, FORMAT_RGBA32F, FORMAT_RGBA8_UNORM, FORMAT_RGB10A2_UNORM = 1, 2, 3, 4
+FORMAT_R11G11B10_FLOAT = 5  # input only: 4 B/px, int32 [H, W] tensors with api.image(t, format=FORMAT_R11G11B10_FLOAT)
 FLAG_RCAS_CLAMP, FLAG_EXACT, FLAG_FORCE_DIRECT, FLAG_NO_RCAS, FLAG_H_REFERENCE, FLAG_PRECISE = 1, 2, 4, 8, 16, 32
 FLAG_RCAS_DENOISE, FLAG_RCAS_PASSTHROUGH_ALPHA, FLAG_OUTPUT_SQUARE, FLAG_FUSED, FLAG_RCAS_HX2 = 64, 128, 256, 512, 1024
 FLAG_SRTM_INPUT = 2048

@@ -8,7 +8,7 @@ import ctypes
 import torch
 
 from . import _lib
-from ._lib import FORMAT_RGB10A2_UNORM, FORMAT_RGBA8_UNORM  # noqa: F401
+from ._lib import FORMAT_R11G11B10_FLOAT, FORMAT_RGB10A2_UNORM, FORMAT_RGBA8_UNORM  # noqa: F401
 from ._lib import FLAG_FUSED, FLAG_OUTPUT_SQUARE, FLAG_RCAS_HX2, FLAG_SRTM_INPUT  # noqa: F401
 from ._lib import POST_LFGA, POST_SRTM_INVERSE, POST_TEPD10, POST_TEPD8  # noqa: F401
 from ._lib import (FLAG_EXACT, FLAG_FORCE_DIRECT, FLAG_H_REFERENCE, FLAG_NO_RCAS, FLAG_PRECISE, FLAG_RCAS_DENOISE, FLAG_RCAS_PASSTHROUGH_ALPHA, FLAG_RCAS_CLAMP, FORMAT_RGBA16F,  # noqa: F401
@@ -50,12 +50,17 @@ def easu_input_rows(con, in_height, y0, y1):
     return a.value, b.value
 
 
-def image(t, height=None, row0=0):
-    """Describe tensor `t` ([rows, W, 4]) as logical rows [row0, row0+rows) of an image `height` rows tall."""
+def image(t, height=None, row0=0, format=None):
+    """Describe tensor `t` ([rows, W, 4]) as logical rows [row0, row0+rows) of an image `height` rows tall.
+    An int32 [rows, W] tensor is RGB10A2_UNORM, or R11G11B10_FLOAT (an input format only) with format=FORMAT_R11G11B10_FLOAT."""
     if not t.is_cuda:
         raise Fsr1Error("fsr1 kernels run on CUDA tensors only (no CPU path)")
-    if t.dim() == 2 and t.dtype == torch.int32 and t.stride(1) == 1:      # R10G10B10A2_UNORM: one int32 per pixel
-        fmt = FORMAT_RGB10A2_UNORM
+    if format not in (None, FORMAT_R11G11B10_FLOAT):
+        raise Fsr1Error("format: None (from the tensor) or FORMAT_R11G11B10_FLOAT")
+    if format == FORMAT_R11G11B10_FLOAT and not (t.dim() == 2 and t.dtype == torch.int32 and t.stride(1) == 1):
+        raise Fsr1Error("R11G11B10_FLOAT images are [rows, width] int32 tensors (one 32-bit code per pixel)")
+    if t.dim() == 2 and t.dtype == torch.int32 and t.stride(1) == 1:      # one 32-bit code per pixel
+        fmt = FORMAT_R11G11B10_FLOAT if format == FORMAT_R11G11B10_FLOAT else FORMAT_RGB10A2_UNORM
     else:
         if t.dim() != 3 or t.shape[2] != 4 or t.stride(2) != 1 or t.stride(1) != 4:
             raise Fsr1Error("image tensors must be [rows, width, 4] with contiguous pixels (or [rows, width] int32 for RGB10A2)")
@@ -254,7 +259,8 @@ def launch_count():
 
 
 class HostContext:
-    """fsr1_context_*: owns the intermediate and device staging; frames live in (pinned) host memory."""
+    """fsr1_context_*: owns the intermediate and device staging; frames live in (pinned) host memory.
+    fmt: the input's format; the output is in it too, but float16 [H, W, 4] (RGBA16F) for FORMAT_R11G11B10_FLOAT input (int32 [H, W])."""
 
     def __init__(self, in_w, in_h, out_w, out_h, fmt=FORMAT_RGBA16F):
         self._h = ctypes.c_void_p()

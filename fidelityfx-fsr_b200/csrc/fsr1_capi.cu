@@ -45,10 +45,17 @@ int bytes_per_pixel(uint32_t fmt) {
   switch (fmt) {
     case FSR1_FORMAT_RGBA16F: return 8;
     case FSR1_FORMAT_RGBA32F: return 16;
-    case FSR1_FORMAT_RGBA8_UNORM: case FSR1_FORMAT_RGB10A2_UNORM: return 4;
+    case FSR1_FORMAT_RGBA8_UNORM: case FSR1_FORMAT_RGB10A2_UNORM: case FSR1_FORMAT_R11G11B10_FLOAT: return 4;
     default: return 0;
   }
 }
+
+// The format of the image EASU writes from an input of format `fmt`: R11G11B10_FLOAT is an input format only, its EASU output (and
+// every intermediate and output after it) is RGBA16F, the exact superset of its values.
+uint32_t easu_out_format(uint32_t fmt) { return fmt == FSR1_FORMAT_R11G11B10_FLOAT ? (uint32_t)FSR1_FORMAT_RGBA16F : fmt; }
+
+// R11G11B10_FLOAT input runs on the RGBA16F production kernels (and the fast direct kernel); the parity and fp32 paths do not take it
+constexpr uint32_t kR11Refused = FSR1_FLAG_EXACT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_HX2;
 
 int check_image(const fsr1_image* im) {
   if (!im || !im->data || im->width == 0 || im->height == 0 || im->rows == 0) return FSR1_ERR_INVALID_ARGUMENT;
@@ -95,7 +102,7 @@ bool window_holds(const fsr1_image* im, int first, int last) {  // logical rows 
 // so everything those kernels decline is refused here, before any CUDA call, instead of falling back to a kernel that would ignore
 // the flag.  `out`: the image EASU writes (the intermediate, or the output of a fused frame); null when not checked here.
 int srtm_input_check(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], uint32_t flags) {
-  if (in->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
+  if (in->format != FSR1_FORMAT_RGBA16F && in->format != FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
   if (flags & (FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE)) return FSR1_ERR_UNSUPPORTED;
   if (((uintptr_t)in->data & 15) || (in->pitch_bytes & 15)) return FSR1_ERR_UNSUPPORTED;  // TMA
   if (out && (((uintptr_t)out->data & 15) || (out->pitch_bytes & 15))) return FSR1_ERR_UNSUPPORTED;  // 16-byte pixel-pair stores
@@ -122,6 +129,9 @@ int pointwise(int op, const fsr1_image* in, const fsr1_image* aux, const fsr1_im
   if (aux && (rc = check_image(aux)) != FSR1_OK) return rc;
   if (aux && (aux->row0 != 0 || aux->rows != aux->height)) return FSR1_ERR_INVALID_ARGUMENT;  // tiles are whole images
   if (in->width != out->width || in->height != out->height) return FSR1_ERR_INVALID_ARGUMENT;
+  if (in->format == FSR1_FORMAT_R11G11B10_FLOAT || out->format == FSR1_FORMAT_R11G11B10_FLOAT ||
+      (aux && aux->format == FSR1_FORMAT_R11G11B10_FLOAT))
+    return FSR1_ERR_UNSUPPORTED;  // an EASU input format only
   if (y1 == 0) y1 = out->height;
   if (y0 >= y1 || y1 > out->height) return FSR1_ERR_INVALID_ARGUMENT;
   if (!window_holds(out, (int)y0, (int)y1 - 1) || !window_holds(in, (int)y0, (int)y1 - 1)) return FSR1_ERR_WINDOW;
@@ -212,7 +222,9 @@ int fsr1_easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16
   int rc;
   if ((rc = check_image(in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
   if (!con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
-  if (in->format != out->format) return FSR1_ERR_UNSUPPORTED;
+  if (out->format != easu_out_format(in->format)) return FSR1_ERR_UNSUPPORTED;
+  const bool r11 = in->format == FSR1_FORMAT_R11G11B10_FLOAT;
+  if (r11 && (flags & kR11Refused)) return FSR1_ERR_UNSUPPORTED;
   if (y1 == 0) y1 = out->height;
   if (y0 >= y1 || y1 > out->height) return FSR1_ERR_INVALID_ARGUMENT;
   if (!window_holds(out, (int)y0, (int)y1 - 1)) return FSR1_ERR_WINDOW;
@@ -246,6 +258,12 @@ int fsr1_easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16
       p.sync = HaloSync{};
     }
     if (e == cudaErrorNotSupported && srtm_in) return FSR1_ERR_UNSUPPORTED;  // nothing launched; no other kernel applies the flag
+  } else if (r11 && !(flags & FSR1_FLAG_FORCE_DIRECT)) {  // the RGBA16F kernels' R11G11B10_FLOAT variants; else the direct kernel
+    if (t_sync) p.sync = *t_sync;
+    e = launch_easu_h_tiled(p, s, &name, srtm_in, true);
+    if (e == cudaSuccess && t_sync) t_sync_used = true;
+    p.sync = HaloSync{};
+    if (e == cudaErrorNotSupported && srtm_in) return FSR1_ERR_UNSUPPORTED;
   } else if (in->format == FSR1_FORMAT_RGBA32F && !exact && !(flags & FSR1_FLAG_FORCE_DIRECT)) {
     e = launch_easu_f32_tiled(p, s, &name);
   } else if ((in->format == FSR1_FORMAT_RGBA8_UNORM || in->format == FSR1_FORMAT_RGB10A2_UNORM) && !exact &&
@@ -267,7 +285,7 @@ int fsr1_rcas(const fsr1_image* in, const fsr1_image* out, const uint32_t con[4]
   if ((rc = check_image(in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
   if (!con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
   if (flags & FSR1_FLAG_SRTM_INPUT) return FSR1_ERR_INVALID_ARGUMENT;  // RCAS has no input stage
-  if (in->format != out->format) return FSR1_ERR_UNSUPPORTED;
+  if (in->format != out->format || in->format == FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
   if (in->width != out->width || in->height != out->height) return FSR1_ERR_INVALID_ARGUMENT;
   if (y1 == 0) y1 = out->height;
   if (y0 >= y1 || y1 > out->height) return FSR1_ERR_INVALID_ARGUMENT;
@@ -328,10 +346,17 @@ int fsr1_upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
   NvtxRange range("FSR1 upscale");
   if (!out) return FSR1_ERR_INVALID_ARGUMENT;
   if (y1 == 0) y1 = out->height;
+  const bool r11 = in && in->format == FSR1_FORMAT_R11G11B10_FLOAT;
+  if (r11) {  // every image after EASU is RGBA16F; refused here so that no EASU launch precedes a refusal of the RCAS pass
+    if (out->format != FSR1_FORMAT_RGBA16F || (tmp && !(flags & FSR1_FLAG_NO_RCAS) && tmp->format != FSR1_FORMAT_RGBA16F))
+      return FSR1_ERR_UNSUPPORTED;
+    if (flags & kR11Refused) return FSR1_ERR_UNSUPPORTED;
+  }
   if (flags & FSR1_FLAG_NO_RCAS) return fsr1_easu(in, out, easu_con, y0, y1, flags, stream);
   // EASU also produces the one-row apron RCAS reads, so a row slab needs no second exchange
   const uint32_t e0 = y0 == 0 ? 0 : y0 - 1, e1 = y1 >= out->height ? out->height : y1 + 1;
-  if ((flags & FSR1_FLAG_FUSED) && in && easu_con && rcas_con && in->format == FSR1_FORMAT_RGBA16F && out->format == FSR1_FORMAT_RGBA16F &&
+  if ((flags & FSR1_FLAG_FUSED) && in && easu_con && rcas_con && (in->format == FSR1_FORMAT_RGBA16F || r11) &&
+      out->format == FSR1_FORMAT_RGBA16F &&
       !(flags & (FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_CLAMP |
                  FSR1_FLAG_RCAS_DENOISE | FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA | FSR1_FLAG_OUTPUT_SQUARE | FSR1_FLAG_RCAS_HX2))) {
     int rc;
@@ -351,7 +376,7 @@ int fsr1_upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
     p.y0 = (int)y0; p.y1 = (int)y1;
     const char* name = "";
     if (t_sync) p.sync = *t_sync;
-    const cudaError_t e = launch_fused_h(p, rcas_con[1], 0, static_cast<cudaStream_t>(stream), &name, srtm_in);
+    const cudaError_t e = launch_fused_h(p, rcas_con[1], 0, static_cast<cudaStream_t>(stream), &name, srtm_in, r11);
     if (e == cudaSuccess && t_sync) t_sync_used = true;
     if (e == cudaSuccess) {
       t_last_kernel = name;
@@ -397,11 +422,13 @@ int post_params(const fsr1_post* post, uint32_t in_format, uint32_t out_format, 
   if ((rc = post_tile(post->grain, (ops & FSR1_POST_LFGA) != 0, q.grain, q.grain_fmt)) != FSR1_OK) return rc;
   if ((rc = post_tile(post->dither, tepd, q.dither, q.dither_fmt)) != FSR1_OK) return rc;
   if (q.grain_fmt && q.grain_fmt != FSR1_FORMAT_RGBA16F && q.grain_fmt != FSR1_FORMAT_RGBA32F) return FSR1_ERR_UNSUPPORTED;  // signed values
+  if (q.dither_fmt == FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;  // an EASU input format only
   q.ops = (int)ops;
   q.amount = post->lfga_amount;
   q.frame = post->frame;
-  // formats: RGBA16F in; RGBA16F out, or with TEPD the matching UNORM code values (the rule of fsr1_tepd)
-  if (in_format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
+  // formats: RGBA16F or R11G11B10_FLOAT in; RGBA16F out, or with TEPD the matching UNORM code values (the rule of fsr1_tepd)
+  if (in_format != FSR1_FORMAT_RGBA16F && in_format != FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
+  if (in_format == FSR1_FORMAT_R11G11B10_FLOAT && (flags & kR11Refused)) return FSR1_ERR_UNSUPPORTED;
   const uint32_t unorm = (ops & FSR1_POST_TEPD8) ? FSR1_FORMAT_RGBA8_UNORM : (ops & FSR1_POST_TEPD10) ? FSR1_FORMAT_RGB10A2_UNORM : 0;
   if (out_format != FSR1_FORMAT_RGBA16F && (!unorm || out_format != unorm)) return FSR1_ERR_UNSUPPORTED;
   // the half-arithmetic parity paths, fp32 EXACT/direct kernels and EASU-only frames keep the separate passes
@@ -454,7 +481,8 @@ int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_im
   if ((flags & FSR1_FLAG_FUSED) && !(flags & (FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_CLAMP | FSR1_FLAG_RCAS_DENOISE |
                                               FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA | FSR1_FLAG_OUTPUT_SQUARE))) {
     if (t_sync) e.sync = *t_sync;  // sharded frame: the neighbour hand-shake rides inside the kernel, as in fsr1_upscale
-    const cudaError_t err = launch_fused_h_post(e, rcas_con[1], q, (int)out->format, s, &name, srtm_in);
+    const cudaError_t err = launch_fused_h_post(e, rcas_con[1], q, (int)out->format, s, &name, srtm_in,
+                                                in->format == FSR1_FORMAT_R11G11B10_FLOAT);
     if (err == cudaSuccess && t_sync) t_sync_used = true;
     if (err == cudaSuccess) {
       t_last_kernel = name;
@@ -536,7 +564,7 @@ int fsr1_context_create(fsr1_context** ctx, uint32_t in_w, uint32_t in_h, uint32
   if (!c) return FSR1_ERR_INVALID_ARGUMENT;
   memset(c, 0, sizeof *c);
   c->in_w = in_w; c->in_h = in_h; c->out_w = out_w; c->out_h = out_h; c->format = format;
-  const uint64_t bpp = (uint64_t)bytes_per_pixel(format);
+  const uint64_t bpp = (uint64_t)bytes_per_pixel(easu_out_format(format));  // the intermediate
   c->tmp_pitch = ((uint64_t)out_w * bpp + 127) & ~(uint64_t)127;
   cudaError_t e = cudaMalloc(&c->tmp, c->tmp_pitch * out_h);
   if (e != cudaSuccess) { delete c; return cuda_fail(e); }
@@ -557,8 +585,8 @@ static int context_run(fsr1_context* c, void* in_dev, uint64_t in_pitch, void* o
   if (render_w == 0) render_w = c->in_w;
   if (render_h == 0) render_h = c->in_h;
   fsr1_image in = {in_dev, in_pitch, render_w, render_h, 0, render_h, c->format, 0};
-  fsr1_image tmp = {c->tmp, c->tmp_pitch, c->out_w, c->out_h, 0, c->out_h, c->format, 0};
-  fsr1_image out = {out_dev, out_pitch, c->out_w, c->out_h, 0, c->out_h, c->format, 0};
+  fsr1_image tmp = {c->tmp, c->tmp_pitch, c->out_w, c->out_h, 0, c->out_h, easu_out_format(c->format), 0};
+  fsr1_image out = {out_dev, out_pitch, c->out_w, c->out_h, 0, c->out_h, easu_out_format(c->format), 0};
   uint32_t econ[16], rcon[4];
   // exactly what FSR_Filter::Upscale passes (sample/src/DX12/FSR_Filter.cpp:106,124)
   fsr1_easu_con(econ, (float)render_w, (float)render_h, (float)render_w, (float)render_h, (float)c->out_w, (float)c->out_h);
@@ -578,7 +606,7 @@ int fsr1_context_upscale_render(fsr1_context* c, const void* in_dev, uint64_t in
 int fsr1_context_upscale_post(fsr1_context* c, const void* in_dev, uint64_t in_pitch, uint32_t render_w, uint32_t render_h,
                               void* out_dev, uint64_t out_pitch, float sharpness, const fsr1_post* post, uint32_t flags, void* stream) {
   if (!c || !in_dev || !out_dev) return FSR1_ERR_INVALID_ARGUMENT;
-  if (c->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
+  if (c->format != FSR1_FORMAT_RGBA16F && c->format != FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
   if (render_w == 0) render_w = c->in_w;
   if (render_h == 0) render_h = c->in_h;
   if (render_w > c->in_w || render_h > c->in_h) return FSR1_ERR_INVALID_ARGUMENT;  // would read past the caller's input
@@ -588,7 +616,7 @@ int fsr1_context_upscale_post(fsr1_context* c, const void* in_dev, uint64_t in_p
   if ((ops & FSR1_POST_TEPD10) && !(ops & FSR1_POST_TEPD8)) ofmt = FSR1_FORMAT_RGB10A2_UNORM;
   if ((ops & FSR1_POST_TEPD8) && !(ops & FSR1_POST_TEPD10)) ofmt = FSR1_FORMAT_RGBA8_UNORM;
   fsr1_image in = {const_cast<void*>(in_dev), in_pitch, render_w, render_h, 0, render_h, c->format, 0};
-  fsr1_image tmp = {c->tmp, c->tmp_pitch, c->out_w, c->out_h, 0, c->out_h, c->format, 0};
+  fsr1_image tmp = {c->tmp, c->tmp_pitch, c->out_w, c->out_h, 0, c->out_h, FSR1_FORMAT_RGBA16F, 0};
   fsr1_image out = {out_dev, out_pitch, c->out_w, c->out_h, 0, c->out_h, ofmt, 0};
   uint32_t econ[16], rcon[4];
   fsr1_easu_con(econ, (float)render_w, (float)render_h, (float)render_w, (float)render_h, (float)c->out_w, (float)c->out_h);
@@ -605,12 +633,12 @@ int fsr1_context_upscale(fsr1_context* c, const void* in_dev, uint64_t in_pitch,
 int fsr1_context_upscale_host(fsr1_context* c, const void* in_host, uint64_t in_pitch, void* out_host,
                               uint64_t out_pitch, float sharpness, uint32_t flags, void* stream) {
   if (!c || !in_host || !out_host) return FSR1_ERR_INVALID_ARGUMENT;
-  const uint64_t bpp = (uint64_t)bytes_per_pixel(c->format);
-  if (in_pitch < c->in_w * bpp || out_pitch < c->out_w * bpp) return FSR1_ERR_INVALID_ARGUMENT;
+  const uint64_t bpp = (uint64_t)bytes_per_pixel(c->format), obpp = (uint64_t)bytes_per_pixel(easu_out_format(c->format));
+  if (in_pitch < c->in_w * bpp || out_pitch < c->out_w * obpp) return FSR1_ERR_INVALID_ARGUMENT;
   cudaError_t e;
   if (!c->dev_in || !c->dev_out) {  // both or neither: a failed second allocation leaves nothing half-initialised
     c->in_pitch = ((uint64_t)c->in_w * bpp + 127) & ~(uint64_t)127;
-    c->out_pitch = ((uint64_t)c->out_w * bpp + 127) & ~(uint64_t)127;
+    c->out_pitch = ((uint64_t)c->out_w * obpp + 127) & ~(uint64_t)127;
     void *din = nullptr, *dout = nullptr;
     if ((e = cudaMalloc(&din, c->in_pitch * c->in_h)) != cudaSuccess) return cuda_fail(e);
     if ((e = cudaMalloc(&dout, c->out_pitch * c->out_h)) != cudaSuccess) { cudaFree(din); return cuda_fail(e); }
@@ -622,7 +650,7 @@ int fsr1_context_upscale_host(fsr1_context* c, const void* in_host, uint64_t in_
   if (e != cudaSuccess) return cuda_fail(e);
   int rc = context_run(c, c->dev_in, c->in_pitch, c->dev_out, c->out_pitch, sharpness, flags, stream);
   if (rc != FSR1_OK) return rc;
-  e = cudaMemcpy2DAsync(out_host, out_pitch, c->dev_out, c->out_pitch, c->out_w * bpp, c->out_h, cudaMemcpyDeviceToHost, s);
+  e = cudaMemcpy2DAsync(out_host, out_pitch, c->dev_out, c->out_pitch, c->out_w * obpp, c->out_h, cudaMemcpyDeviceToHost, s);
   if (e != cudaSuccess) return cuda_fail(e);
   return FSR1_OK;
 }

@@ -166,6 +166,23 @@ template <> struct Px<Unorm10> {
   }
 };
 
+// R11G11B10_FLOAT (DXGI_FORMAT_R11G11B10_FLOAT, 4 B/px): bits 0-10 R, 11-21 G (6 mantissa bits below 5 exponent bits), 22-31 B
+// (5 mantissa bits below 5 exponent bits).  Each channel is a half without its sign bit and with the low mantissa bits cut off (same
+// exponent and bias), so the texel decodes EXACTLY to the RGBA16F texel (R, G, B, 1.0) with shifts and masks: (e << 10) | (m << 4)
+// for R and G, (e << 10) | (m << 5) for B; denormals, inf and NaN land on their half counterparts.  An input format only.
+struct R11f {};
+__host__ __device__ __forceinline__ uint2 r11_to_half(uint32_t v) {
+  return make_uint2(((v & 0x7ffu) << 4) | ((v << 9) & 0x7ff00000u), ((v >> 17) & 0x7fe0u) | 0x3c000000u);
+}
+template <> struct Px<R11f> {
+  static constexpr int kBytes = 4;
+  static __device__ __forceinline__ float3 load(const ImgView& im, int x, int y) {
+    const uint2 v = r11_to_half(__ldg(reinterpret_cast<const uint32_t*>(im.base + (long long)(y - im.row0) * im.pitch) + x));
+    const float2 rg = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+    return make_float3(rg.x, rg.y, __low2float(*reinterpret_cast<const __half2*>(&v.y)));
+  }
+};
+
 // c / (2^n - 1) CORRECTLY ROUNDED without a division: q = c * (1/s) is off by one ulp for half of the 8-bit codes, and an ulp of
 // luma is enough to turn an exact tie between neighbouring texels (0/0 in FsrEasuSetF's length term, ffx_fsr1.h:298) into 1.0 instead
 // of 0.0 — the filter of a whole 2x2 cell block changes.  One FMA refinement makes q exact for every 8- and 10-bit code
@@ -253,13 +270,15 @@ cudaError_t launch_rcas_direct(const RcasParams& p, int format, bool exact, cuda
 // Packed-half production kernels.  Return cudaErrorNotSupported when the image layout does not
 // meet their alignment needs (the caller then falls back to the direct kernels).  srtm_in: FSR1_FLAG_SRTM_INPUT (the caller
 // must not fall back then: no other kernel applies it).
-cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in = false);
+// r11: the input is R11G11B10_FLOAT (the output RGBA16F); no fall-back either (launch_easu_direct decodes the format itself).
+cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in = false, bool r11 = false);
 cudaError_t launch_rcas_h_packed(const RcasParams& p, cudaStream_t s, const char** name);
 // UNORM images through the TMA-tiled 2x EASU / packed RCAS kernels: cudaErrorNotSupported when not applicable
 cudaError_t launch_easu_u_tiled(const EasuParams& p, int format, cudaStream_t s, const char** name);
 cudaError_t launch_rcas_u_packed(const RcasParams& p, int format, cudaStream_t s, const char** name);
 // EASU -> RCAS in one kernel (RGBA16F, exactly 2x, out-of-image taps read 0): e.in = input, e.out = final output, rows [e.y0, e.y1)
-cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in = false);
+cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in = false,
+                           bool r11 = false);
 cudaError_t launch_easu_f32_tiled(const EasuParams& p, cudaStream_t s, const char** name);  // RGBA32F, exactly 2x
 cudaError_t launch_easu_h_precise(const EasuParams& p, cudaStream_t s, const char** name);  // RGBA16F io, fp32 math, 2x
 cudaError_t launch_rcas_f32_packed(const RcasParams& p, cudaStream_t s, const char** name);

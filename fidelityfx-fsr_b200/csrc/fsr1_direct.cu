@@ -63,8 +63,9 @@ template <bool kExact> __device__ __forceinline__ float luma(float3 c) {
   return A::add(A::mul(c.z, 0.5f), A::add(A::mul(c.x, 0.5f), c.y));  // 2*luma = 0.5B + (0.5R + G)
 }
 
-template <typename S, bool kExact>
-__global__ void __launch_bounds__(256) easu_direct_kernel(const EasuParams p) {
+// S: the input's storage, SO: the output's (the same but for R11G11B10_FLOAT input, which writes RGBA16F)
+template <typename S, typename SO, bool kExact>
+__device__ __forceinline__ void easu_direct_body(const EasuParams& p) {
   using A = Ar<kExact>;
   const int ox = blockIdx.x * 32 + threadIdx.x;
   const int oy = p.y0 + blockIdx.y * 8 + threadIdx.y;
@@ -128,9 +129,17 @@ __global__ void __launch_bounds__(256) easu_direct_kernel(const EasuParams p) {
   const float mnR = fminf(fminf(f.x, fminf(g.x, j.x)), k.x), mxR = fmaxf(fmaxf(f.x, fmaxf(g.x, j.x)), k.x);
   const float mnG = fminf(fminf(f.y, fminf(g.y, j.y)), k.y), mxG = fmaxf(fmaxf(f.y, fmaxf(g.y, j.y)), k.y);
   const float mnB = fminf(fminf(f.z, fminf(g.z, j.z)), k.z), mxB = fmaxf(fmaxf(f.z, fmaxf(g.z, j.z)), k.z);
-  Px<S>::store(p.out, ox, oy, fminf(mxR, fmaxf(mnR, A::mul(aC.x, rW))), fminf(mxG, fmaxf(mnG, A::mul(aC.y, rW))),
-               fminf(mxB, fmaxf(mnB, A::mul(aC.z, rW))));
+  Px<SO>::store(p.out, ox, oy, fminf(mxR, fmaxf(mnR, A::mul(aC.x, rW))), fminf(mxG, fmaxf(mnG, A::mul(aC.y, rW))),
+                fminf(mxB, fmaxf(mnB, A::mul(aC.z, rW))));
 }
+
+template <typename S, bool kExact>
+__global__ void __launch_bounds__(256) easu_direct_kernel(const EasuParams p) {
+  easu_direct_body<S, S, kExact>(p);
+}
+
+// R11G11B10_FLOAT input: every texel decoded exactly (r11_to_half) to fp32; the output is RGBA16F
+__global__ void __launch_bounds__(256) easu_direct_r11_kernel(const EasuParams p) { easu_direct_body<R11f, __half, false>(p); }
 
 template <typename S>
 __device__ __forceinline__ float3 rcas_fetch(const RcasParams& p, int x, int y) {
@@ -225,6 +234,11 @@ cudaError_t launch_easu_direct(const EasuParams& p, int format, bool exact, cuda
     case 2: launch_easu_s<float>(p, exact, s, grid, block); break;
     case 3: launch_easu_s<Unorm8>(p, exact, s, grid, block); break;
     case 4: launch_easu_s<Unorm10>(p, exact, s, grid, block); break;
+    case 5:
+      if (exact) return cudaErrorNotSupported;  // refused by the caller (FSR1_FLAG_EXACT is an fp32-image path)
+      easu_direct_r11_kernel<<<grid, block, 0, s>>>(p);
+      *name = "easu_direct<r11g11b10f_in,f16out,fast>";
+      return cudaGetLastError();
     default: return cudaErrorInvalidValue;
   }
   *name = direct_name("easu", format, exact);

@@ -32,6 +32,7 @@
 // them, as it does the tap loop's reads.
 #include "fsr1_easu_quad.cuh"
 #include "fsr1_post.cuh"
+#include "fsr1_r11.cuh"
 
 namespace fsr1 {
 
@@ -146,7 +147,10 @@ __host__ __device__ inline size_t pairs_smem_bytes(int BW, int BH) {
   return off + 16 + 128;  // + barriers + slack for the manual 128B alignment
 }
 
-template <bool kSrtmIn = false>
+// kR11: R11G11B10_FLOAT input (fsr1_r11.cuh): the box is BW4 = BW + 2 or + 4 texels wide (a multiple of 4), from the multiple of 4 at or
+// before the half tile's origin.  BW * BH <= kR11Per * kThreads holds for every upscale (BW <= 68, BH <= 35; the launcher checks).
+constexpr int kR11Per = 10;
+template <bool kSrtmIn = false, bool kR11 = false>
 __global__ void __launch_bounds__(kThreads, 3)
 easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap, const int BW, const int BH,
                     const int tiles_x, const int n_tiles) {
@@ -186,8 +190,8 @@ easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap
   if (tid == 0 && t < n_tiles) {
     int a, b, fx, fy;
     origin(t, a, b, fx, fy);
-    mbar_expect_tx(&bar[0], (uint32_t)n * 8u);
-    tma_load_2d(base, &tmap, fx, fy - p.in.row0, &bar[0]);
+    mbar_expect_tx(&bar[0], kR11 ? (uint32_t)(((BW + 5) & ~3) * BH) * 4u : (uint32_t)n * 8u);
+    tma_load_2d(base, &tmap, kR11 ? fx & ~3 : fx, fy - p.in.row0, &bar[0]);
   }
   for (int it = 0; t < n_tiles; t += gridDim.x, it++) {
   const int bsel = it & 1;
@@ -195,8 +199,8 @@ easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap
     int a, b, fx, fy;
     origin(t + gridDim.x, a, b, fx, fy);
     fence_proxy_async();
-    mbar_expect_tx(&bar[bsel ^ 1], (uint32_t)n * 8u);
-    tma_load_2d(base + (bsel ^ 1) * tstride, &tmap, fx, fy - p.in.row0, &bar[bsel ^ 1]);
+    mbar_expect_tx(&bar[bsel ^ 1], kR11 ? (uint32_t)(((BW + 5) & ~3) * BH) * 4u : (uint32_t)n * 8u);
+    tma_load_2d(base + (bsel ^ 1) * tstride, &tmap, kR11 ? fx & ~3 : fx, fy - p.in.row0, &bar[bsel ^ 1]);
   }
   uint2* tile = reinterpret_cast<uint2*>(base + bsel * tstride);
   int ox0, oy0, fx0, fy0;
@@ -204,15 +208,20 @@ easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap
   mbar_wait(&bar[bsel], (it >> 1) & 1);
 
   if (fx0 < 0 || fy0 < 0 || fx0 + BW > p.in.w || fy0 + BH > p.in.h) {  // border tiles only (CTA-uniform)
-    clamp_fixup(tile, BW, BW, BH, fx0, fy0, p.in.w, p.in.h, lane, warp, kThreads / 32);
+    if constexpr (kR11) clamp_fixup(reinterpret_cast<uint32_t*>(tile) + (fx0 & 3), (BW + 5) & ~3, BW, BH, fx0, fy0, p.in.w, p.in.h, lane, warp, kThreads / 32);
+    else clamp_fixup(tile, BW, BW, BH, fx0, fy0, p.in.w, p.in.h, lane, warp, kThreads / 32);
     fence_proxy_async();
     __syncthreads();
   }
 
-  for (int i = tid; i < n; i += kThreads) {  // phase 1
-    uint2 c = tile[i];
-    if (kSrtmIn) tile[i] = c = srtm_texel(c);
-    L[i] = texel_luma(c);
+  if constexpr (kR11) {
+    r11_phase1_inplace<kSrtmIn, kThreads, kR11Per>(tile, L, n, BW, (BW + 5) & ~3, fx0 & 3, tid);
+  } else {
+    for (int i = tid; i < n; i += kThreads) {  // phase 1
+      uint2 c = tile[i];
+      if (kSrtmIn) tile[i] = c = srtm_texel(c);
+      L[i] = texel_luma(c);
+    }
   }
   __syncthreads();
 
@@ -264,6 +273,7 @@ easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap
   halo_sync_end(p.sync);
 }
 
+
 // =======================================================================================================
 //  2x kernel: lane = the quad of output pixels sharing input cell (k,m); persistent, double-buffered TMA
 // =======================================================================================================
@@ -274,13 +284,22 @@ template <int NW> struct __align__(128) QuadSmem {
   uint64_t bar[2];
 };
 
-template <int NW, int MINB, bool kSrtmIn = false>
-__global__ void __launch_bounds__(NW * 32, MINB)
-easu_h_quad2x_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap, const int tiles_x,
-                     const int n_tiles, const int mbase) {
+// kR11: R11G11B10_FLOAT input (fsr1_r11.cuh): a kUBW = 40 texel box from 2 texels left of the half tile's origin (32 tx - 4: 16 bytes)
+constexpr int kUBW = kQBW + 4;
+template <int NW, bool kSrtmIn, bool kR11>
+__device__ __forceinline__ void quad_body(const EasuParams p, const CUtensorMap& tmap, const int tiles_x, const int n_tiles,
+                                          const int mbase) {
   using C = QuadCfg<NW>;
   constexpr int NT = NW * 32;
+  constexpr uint32_t kBoxBytes = kR11 ? kUBW * C::kBH * 4u : C::kElems * 8u;
+  constexpr int kShift = kR11 ? 2 : 0;
+  constexpr int kStage = ((kUBW * C::kBH * 4 + 127) / 128) * 128 / 4;
   __shared__ QuadSmem<NW> sm;
+  uint32_t* stage = nullptr;  // kR11: where the boxes land (fsr1_r11.cuh)
+  if constexpr (kR11) {
+    __shared__ R11Stage<kStage> r11_stage;
+    stage = &r11_stage.w[0][0];
+  }
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid == 0) {
     mbar_init(&sm.bar[0], 1);
@@ -295,8 +314,8 @@ easu_h_quad2x_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tma
   int tx = t % tiles_x, ty = t / tiles_x;
   const int step_x = (int)gridDim.x % tiles_x, step_y = (int)gridDim.x / tiles_x;
   if (tid == 0 && t < n_tiles) {
-    mbar_expect_tx(&sm.bar[0], C::kElems * 8u);
-    tma_load_2d(sm.tile[0], &tmap, tx * kQCX - 2, mbase + ty * C::kCY - 1 - p.in.row0, &sm.bar[0]);
+    mbar_expect_tx(&sm.bar[0], kBoxBytes);
+    tma_load_2d(kR11 ? (void*)stage : (void*)sm.tile[0], &tmap, tx * kQCX - 2 - kShift, mbase + ty * C::kCY - 1 - p.in.row0, &sm.bar[0]);
   }
   for (int it = 0; t < n_tiles; t += gridDim.x, it++) {
     const int b = it & 1;
@@ -304,23 +323,29 @@ easu_h_quad2x_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tma
     if (txn >= tiles_x) { txn -= tiles_x; tyn++; }
     if (tid == 0 && t + (int)gridDim.x < n_tiles) {  // prefetch it into the other buffer (its readers all passed
       fence_proxy_async();                           // the barrier that closed the previous iteration)
-      mbar_expect_tx(&sm.bar[b ^ 1], C::kElems * 8u);
-      tma_load_2d(sm.tile[b ^ 1], &tmap, txn * kQCX - 2, mbase + tyn * C::kCY - 1 - p.in.row0, &sm.bar[b ^ 1]);
+      mbar_expect_tx(&sm.bar[b ^ 1], kBoxBytes);
+      tma_load_2d(kR11 ? (void*)(stage + (b ^ 1) * kStage) : (void*)sm.tile[b ^ 1], &tmap, txn * kQCX - 2 - kShift,
+                  mbase + tyn * C::kCY - 1 - p.in.row0, &sm.bar[b ^ 1]);
     }
-    uint2* tile = sm.tile[b];
+    uint2* tile = sm.tile[kR11 ? 0 : b];  // kR11: phase 1 writes the half tile after the previous tile's closing barrier
     const int gx0 = tx * kQCX - 2, gy0 = mbase + ty * C::kCY - 1;
     tx = txn;
     ty = tyn;
     mbar_wait(&sm.bar[b], (it >> 1) & 1);
     if (gx0 < 0 || gy0 < 0 || gx0 + kQBW > p.in.w || gy0 + C::kBH > p.in.h) {
-      clamp_fixup(tile, kQBW, kQBW, C::kBH, gx0, gy0, p.in.w, p.in.h, lane, warp, NW);
+      if constexpr (kR11) clamp_fixup(stage + b * kStage + kShift, kUBW, kQBW, C::kBH, gx0, gy0, p.in.w, p.in.h, lane, warp, NW);
+      else clamp_fixup(tile, kQBW, kQBW, C::kBH, gx0, gy0, p.in.w, p.in.h, lane, warp, NW);
       fence_proxy_async();  // these generic-proxy writes are later overwritten by a TMA (async proxy) load
       __syncthreads();
     }
-    for (int i = tid; i < C::kElems; i += NT) {
-      uint2 c = tile[i];
-      if (kSrtmIn) tile[i] = c = srtm_texel(c);
-      sm.L[i] = texel_luma(c);
+    if constexpr (kR11) {
+      r11_phase1_staged<kSrtmIn, NT>(stage + b * kStage, tile, sm.L, C::kElems, kQBW, kUBW, kShift, tid);
+    } else {
+      for (int i = tid; i < C::kElems; i += NT) {
+        uint2 c = tile[i];
+        if (kSrtmIn) tile[i] = c = srtm_texel(c);
+        sm.L[i] = texel_luma(c);
+      }
     }
     __syncthreads();
     for (int idx = tid; idx < kQSW * C::kSH; idx += NT) {
@@ -344,11 +369,23 @@ easu_h_quad2x_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tma
   halo_sync_end(p.sync);
 }
 
+template <int NW, int MINB, bool kSrtmIn = false>
+__global__ void __launch_bounds__(NW * 32, MINB)
+easu_h_quad2x_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap, const int tiles_x,
+                     const int n_tiles, const int mbase) {
+  quad_body<NW, kSrtmIn, false>(p, tmap, tiles_x, n_tiles, mbase);
+}
+template <int NW, int MINB, bool kSrtmIn>
+__global__ void __launch_bounds__(NW * 32, MINB)
+easu_r11_quad2x_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap, const int tiles_x,
+                       const int n_tiles, const int mbase) {
+  quad_body<NW, kSrtmIn, true>(p, tmap, tiles_x, n_tiles, mbase);
+}
+
 // ---- 2x EASU for the UNORM formats the sample renders into (sample/src/DX12/FSR_Filter.cpp:72-73) -------------------
 // Same phases as easu_h_quad2x_kernel.  The TMA box holds 4-byte texels (origin rounded down to 4 texels = 16 bytes, so
 // the box is 40 wide); one pass decodes it (c / (2^n - 1), fp32) into the half tile the tap loop reads and into the
 // fp32 luma plane; the epilogue re-encodes in the half domain (StoreUnorm).
-constexpr int kUBW = kQBW + 4;
 template <int NW> struct __align__(128) QuadSmemU {
   uint32_t stage[2][((kUBW * QuadCfg<NW>::kBH * 4 + 127) / 128) * 128 / 4];
   uint2 tile[QuadCfg<NW>::kPad];
@@ -493,12 +530,13 @@ cudaError_t launch_easu_u_tiled(const EasuParams& p, int format, cudaStream_t s,
   return cudaGetLastError();
 }
 
-cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in) {
+cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in, bool r11) {
   // layout requirements of TMA and of the vector stores
   if ((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15) || (reinterpret_cast<uintptr_t>(p.out.base) & 15) ||
       (p.out.pitch & 15))
     return cudaErrorNotSupported;
   CUtensorMap tmap;
+  const CUtensorMapDataType type = r11 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT64;
 
   if (is_2x(p)) {
     // 4 warps x 7 CTAs per SM: the kernel needs 72 registers, exactly what 7 x 128 threads allow.  A launch that waits
@@ -506,9 +544,15 @@ cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char*
     // registers are taken but 256, so the one-warp halo_push_kernel that the wait depends on cannot be placed beside a
     // grid that fills every SM, and ranks sharing one GPU would wait for each other until the spin timeout.
     constexpr int NW = 4, CY = 2 * NW;
-    if (!make_tmap(&tmap, p.in, kQBW, CY + 3)) return cudaErrorNotSupported;
+    if (!make_tmap(&tmap, p.in, r11 ? kUBW : kQBW, CY + 3, type)) return cudaErrorNotSupported;
     const QuadGrid g = quad_grid(p, CY, (p.sync.ready[0] || p.sync.ready[1]) ? 6 : 7);
-    if (srtm_in) {
+    if (r11 && srtm_in) {
+      easu_r11_quad2x_kernel<NW, 7, true><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
+      *name = "easu_h_quad2x<4w,7/sm,tma2,r11g11b10f_in,srtm_in>";
+    } else if (r11) {
+      easu_r11_quad2x_kernel<NW, 7, false><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
+      *name = "easu_h_quad2x<4w,7/sm,tma2,r11g11b10f_in>";
+    } else if (srtm_in) {
       easu_h_quad2x_kernel<NW, 7, true><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
       *name = "easu_h_quad2x<4w,7/sm,tma2,srtm_in>";
     } else {
@@ -523,25 +567,24 @@ cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char*
   int BH = max_footprint(p.y1, p.y0, kTileH, p.c0y, p.c0w, false);
   BW = (BW + 1) & ~1;  // inner box extent must be a multiple of 16 bytes
   if (BW > 256 || BH > 256) return cudaErrorNotSupported;
+  if (r11 && BW * BH > kR11Per * kThreads) return cudaErrorNotSupported;  // cannot happen when upscaling (pairs_body)
   const size_t smem = pairs_smem_bytes(BW, BH);
   if (smem > 200 * 1024) return cudaErrorNotSupported;
-  if (!make_tmap(&tmap, p.in, BW, BH)) return cudaErrorNotSupported;
+  if (!make_tmap(&tmap, p.in, r11 ? (BW + 5) & ~3 : BW, BH, type)) return cudaErrorNotSupported;
+  void (*kernel)(const EasuParams, const CUtensorMap, const int, const int, const int, const int) =
+      r11 ? (srtm_in ? easu_h_pairs_kernel<true, true> : easu_h_pairs_kernel<false, true>)
+          : (srtm_in ? easu_h_pairs_kernel<true, false> : easu_h_pairs_kernel<false, false>);
   if (smem > 48 * 1024) {  // per device and cheap: set on every launch that needs the opt-in
-    cudaError_t e = srtm_in ? cudaFuncSetAttribute(easu_h_pairs_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                            : cudaFuncSetAttribute(easu_h_pairs_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
   const int tiles_x = (p.out.w + kTileW - 1) / kTileW, n_tiles = tiles_x * ((p.y1 - p.y0 + kTileH - 1) / kTileH);
   int per_sm = 3;
   while (per_sm > 1 && (size_t)per_sm * (smem + 1024) > 220 * 1024) per_sm--;
   const int grid = n_tiles < per_sm * sm_count() ? n_tiles : per_sm * sm_count();
-  if (srtm_in) {
-    easu_h_pairs_kernel<true><<<grid, kThreads, smem, s>>>(p, tmap, BW, BH, tiles_x, n_tiles);
-    *name = "easu_h_vpairs<64x32,persistent,tma2,srtm_in>";
-  } else {
-    easu_h_pairs_kernel<false><<<grid, kThreads, smem, s>>>(p, tmap, BW, BH, tiles_x, n_tiles);
-    *name = "easu_h_vpairs<64x32,persistent,tma2>";
-  }
+  kernel<<<grid, kThreads, smem, s>>>(p, tmap, BW, BH, tiles_x, n_tiles);
+  *name = r11 ? (srtm_in ? "easu_h_vpairs<64x32,persistent,tma2,r11g11b10f_in,srtm_in>" : "easu_h_vpairs<64x32,persistent,tma2,r11g11b10f_in>")
+              : (srtm_in ? "easu_h_vpairs<64x32,persistent,tma2,srtm_in>" : "easu_h_vpairs<64x32,persistent,tma2>");
   return cudaGetLastError();
 }
 

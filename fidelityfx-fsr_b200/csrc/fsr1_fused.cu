@@ -28,8 +28,11 @@
 // kSrtmIn (FSR1_FLAG_SRTM_INPUT): phase 1 of a step first replaces each texel it covers by FsrSrtmF of it, rounded to half, as
 // easu_h_quad2x_kernel does (fsr1_easu_tiled.cu: after clamp_fixup, luma from the half texel; the fence_proxy_async before the next
 // TMA load into the buffer orders the stores).  Those kFBW (n + 3) texels are exactly the ones the step's taps read.
+// kR11 (R11G11B10_FLOAT input, fsr1_r11.cuh): a kRBW = 40 texel box of 4-byte texels from the multiple of 4 at or before box_x (38
+// texels are 152 bytes: TMA boxes are multiples of 16 bytes), expanded in phase 1 into the same half tile, the step's kFBW (n + 3) texels.
 #include "fsr1_easu_quad.cuh"
 #include "fsr1_post.cuh"
+#include "fsr1_r11.cuh"
 #include "fsr1_rcas_math.cuh"
 
 namespace fsr1 {
@@ -37,6 +40,7 @@ namespace fsr1 {
 constexpr int kFBW = kQBW + 2;   // box width 38: the strip origin 31 tx - 2 is odd for odd tx and TMA boxes start on 16 bytes
 constexpr int kFSW = kFBW - 2;   // texels carrying terms per row
 constexpr int kStripCells = 31;  // cells per strip (lanes 1..31 produce RCAS output; lane 0 only feeds its right neighbour)
+constexpr int kRBW = kFBW + 2;   // kR11: box width in 4-byte texels
 
 struct FusedParams {
   ImgView in, out;
@@ -218,11 +222,18 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
   }
 }
 
-template <int NW, typename SO, bool kSrtmIn>
+template <int NW, typename SO, bool kSrtmIn, bool kR11 = false>
 __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMap& tmap, const PostParams* q) {
   using C = FusedCfg<NW>;
   constexpr int NT = NW * 32, CY = C::kCY;
+  constexpr uint32_t kBoxBytes = kR11 ? kRBW * C::kBH * 4u : C::kElems * 8u;
+  constexpr int kStage = ((kRBW * C::kBH * 4 + 127) / 128) * 128 / 4;
   __shared__ FusedSmem<NW> sm;
+  uint32_t* stage = nullptr;  // kR11: where the boxes land (fsr1_r11.cuh)
+  if constexpr (kR11) {
+    __shared__ R11Stage<kStage> r11_stage;
+    stage = &r11_stage.w[0][0];
+  }
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid == 0) {
     mbar_init(&sm.bar[0], 1);
@@ -236,9 +247,10 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
   FusedStep cur, nxt;
   bool has = iter.next(cur);
   auto box_x = [](const FusedStep& s) { return (kStripCells * s.tx - 2) & ~1; };  // even texel at or before the first tap column
+  auto tma_x = [&](const FusedStep& s) { return kR11 ? box_x(s) & ~3 : box_x(s); };
   if (tid == 0 && has) {
-    mbar_expect_tx(&sm.bar[0], C::kElems * 8u);
-    tma_load_2d(sm.tile[0], &tmap, box_x(cur), cur.m0 - 1 - p.in.row0, &sm.bar[0]);
+    mbar_expect_tx(&sm.bar[0], kBoxBytes);
+    tma_load_2d(kR11 ? (void*)stage : (void*)sm.tile[0], &tmap, tma_x(cur), cur.m0 - 1 - p.in.row0, &sm.bar[0]);
   }
   const __half2 sharp = uh2(p.sharp_h2);
   for (int it = 0; has; it++) {
@@ -246,24 +258,30 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
     const bool hasn = iter.next(nxt);
     if (tid == 0 && hasn) {  // prefetch the next step's box into the other buffer (its readers passed the closing barrier)
       fence_proxy_async();
-      mbar_expect_tx(&sm.bar[b ^ 1], C::kElems * 8u);
-      tma_load_2d(sm.tile[b ^ 1], &tmap, box_x(nxt), nxt.m0 - 1 - p.in.row0, &sm.bar[b ^ 1]);
+      mbar_expect_tx(&sm.bar[b ^ 1], kBoxBytes);
+      tma_load_2d(kR11 ? (void*)(stage + (b ^ 1) * kStage) : (void*)sm.tile[b ^ 1], &tmap, tma_x(nxt), nxt.m0 - 1 - p.in.row0,
+                  &sm.bar[b ^ 1]);
     }
-    uint2* tile = sm.tile[b];
+    uint2* tile = sm.tile[kR11 ? 0 : b];  // kR11: phase 1 writes the half tile after the previous step's closing barrier
     const int k0 = kStripCells * cur.tx - 1;       // first cell of the strip (lane 0)
     const int gxe = box_x(cur), dx = (k0 - 1) - gxe;  // box origin; offset of tap column 0 of lane 0 inside it (0 or 1)
     const int gy0 = cur.m0 - 1, n = cur.n;
     mbar_wait(&sm.bar[b], (it >> 1) & 1);
     if (gxe < 0 || gy0 < 0 || gxe + kFBW > p.in.w || gy0 + C::kBH > p.in.h) {
-      clamp_fixup(tile, kFBW, kFBW, C::kBH, gxe, gy0, p.in.w, p.in.h, lane, warp, NW);
+      if constexpr (kR11) clamp_fixup(stage + b * kStage + (gxe & 3), kRBW, kFBW, C::kBH, gxe, gy0, p.in.w, p.in.h, lane, warp, NW);
+      else clamp_fixup(tile, kFBW, kFBW, C::kBH, gxe, gy0, p.in.w, p.in.h, lane, warp, NW);
       fence_proxy_async();
       __syncthreads();
     }
     // phases 1 and 2 on the rows this step needs (n + 3 texel rows, n + 1 rows of terms)
-    for (int i = tid; i < kFBW * (n + 3); i += NT) {
-      uint2 c = tile[i];
-      if (kSrtmIn) tile[i] = c = srtm_texel(c);
-      sm.L[i] = texel_luma(c);
+    if constexpr (kR11) {
+      r11_phase1_staged<kSrtmIn, NT>(stage + b * kStage, tile, sm.L, kFBW * (n + 3), kFBW, kRBW, gxe & 3, tid);
+    } else {
+      for (int i = tid; i < kFBW * (n + 3); i += NT) {
+        uint2 c = tile[i];
+        if (kSrtmIn) tile[i] = c = srtm_texel(c);
+        sm.L[i] = texel_luma(c);
+      }
     }
     __syncthreads();
     for (int idx = tid; idx < kFSW * (n + 1); idx += NT) {
@@ -305,11 +323,23 @@ fused_h_quad2x_post_kernel(const FusedParams p, const __grid_constant__ CUtensor
   fused_body<NW, SO, kSrtmIn>(p, tmap, &q);
 }
 
+// R11G11B10_FLOAT input: the same two kernels on the kR11 box
+template <int NW, int MINB, bool kSrtmIn>
+__global__ void __launch_bounds__(NW * 32, MINB)
+fused_r11_quad2x_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap) {
+  fused_body<NW, void, kSrtmIn, true>(p, tmap, nullptr);
+}
+template <int NW, int MINB, typename SO, bool kSrtmIn>
+__global__ void __launch_bounds__(NW * 32, MINB)
+fused_r11_quad2x_post_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap, const __grid_constant__ PostParams q) {
+  fused_body<NW, SO, kSrtmIn, true>(p, tmap, &q);
+}
+
 #ifndef FSR1_CPU_EMU
 // tensor map, parameters and grid of a fused launch; cudaErrorNotSupported when the frame is not one the kernel takes.
 // out_align: the alignment the output store needs (16 for RGBA16F pairs, 8 for UNORM pairs).
-static cudaError_t fused_setup(const EasuParams& e, uint32_t sharp_h2, int out_align, CUtensorMap& tmap, FusedParams& p, int& per_sm,
-                               long long& grid) {
+static cudaError_t fused_setup(const EasuParams& e, uint32_t sharp_h2, int out_align, bool r11, CUtensorMap& tmap, FusedParams& p,
+                               int& per_sm, long long& grid) {
   if (!(e.c0x == 0.5f && e.c0y == 0.5f && e.c0z == -0.25f && e.c0w == -0.25f)) return cudaErrorNotSupported;
   if ((reinterpret_cast<uintptr_t>(e.in.base) & 15) || (e.in.pitch & 15) || (reinterpret_cast<uintptr_t>(e.out.base) & (out_align - 1)) ||
       (e.out.pitch & (out_align - 1)))
@@ -320,9 +350,9 @@ static cudaError_t fused_setup(const EasuParams& e, uint32_t sharp_h2, int out_a
   if (!encode) return cudaErrorNotSupported;
   const cuuint64_t dims[2] = {(cuuint64_t)e.in.w, (cuuint64_t)e.in.rows};
   const cuuint64_t strides[1] = {(cuuint64_t)e.in.pitch};
-  const cuuint32_t box[2] = {(cuuint32_t)kFBW, (cuuint32_t)C::kBH};
+  const cuuint32_t box[2] = {(cuuint32_t)(r11 ? kRBW : kFBW), (cuuint32_t)C::kBH};
   const cuuint32_t estr[2] = {1, 1};
-  if (encode(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, e.in.base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  if (encode(&tmap, r11 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, e.in.base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
     return cudaErrorNotSupported;
   p.in = e.in; p.out = e.out; p.y0 = e.y0; p.y1 = e.y1; p.sharp_h2 = sharp_h2; p.sync = e.sync;
@@ -338,15 +368,22 @@ static cudaError_t fused_setup(const EasuParams& e, uint32_t sharp_h2, int out_a
   return cudaSuccess;
 }
 
-cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in) {
+cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in, bool r11) {
   if (clamp) return cudaErrorNotSupported;
   CUtensorMap tmap;
   FusedParams p;
   int per_sm = 7;
   long long grid = 0;
-  const cudaError_t err = fused_setup(e, sharp_h2, 16, tmap, p, per_sm, grid);
+  const cudaError_t err = fused_setup(e, sharp_h2, 16, r11, tmap, p, per_sm, grid);
   if (err != cudaSuccess) return err;
-  if (srtm_in) {
+  if (r11 && srtm_in) {
+    fused_r11_quad2x_kernel<4, 7, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
+    *name = per_sm == 7 ? "fused_easu_rcas_h_quad2x<4w,7/sm,tma2,strips,r11g11b10f_in,srtm_in>"
+                        : "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,r11g11b10f_in,srtm_in>";
+  } else if (r11) {
+    fused_r11_quad2x_kernel<4, 7, false><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
+    *name = per_sm == 7 ? "fused_easu_rcas_h_quad2x<4w,7/sm,tma2,strips,r11g11b10f_in>" : "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,r11g11b10f_in>";
+  } else if (srtm_in) {
     fused_h_quad2x_kernel<4, 7, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
     *name = per_sm == 7 ? "fused_easu_rcas_h_quad2x<4w,7/sm,tma2,strips,srtm_in>" : "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,srtm_in>";
   } else {
@@ -359,42 +396,55 @@ cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cu
 // The display epilogue needs more registers than the 72 of 7 CTAs per SM (-Xptxas -v: DESIGN.md §4): 6 per SM.
 constexpr int kPostPerSm = 6;
 
-cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const PostParams& q, int out_format, cudaStream_t s,
-                                const char** name, bool srtm_in) {
-  CUtensorMap tmap;
-  FusedParams p;
-  int per_sm = kPostPerSm;
-  long long grid = 0;
-  const cudaError_t err = fused_setup(e, sharp_h2, out_format == 1 ? 16 : 8, tmap, p, per_sm, grid);
-  if (err != cudaSuccess) return err;
-  switch (out_format * 2 + (srtm_in ? 1 : 0)) {
-    case 2:
-      fused_h_quad2x_post_kernel<4, kPostPerSm, __half><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
-      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f>";
-      break;
-    case 6:
-      fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm8><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
-      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8>";
-      break;
-    case 8:
-      fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm10><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
-      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2>";
+// the post kernel for out_format (1 RGBA16F, 3 RGBA8_UNORM, 4 RGB10A2_UNORM) and input kind; its name through *name
+template <bool kSrtmIn, bool kR11>
+static cudaError_t launch_post_kernel(const FusedParams& p, const CUtensorMap& tmap, const PostParams& q, int out_format, long long grid,
+                                      cudaStream_t s, const char** name) {
+  static const char* const names[3][4] = {
+      {"fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f>", "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f,srtm_in>",
+       "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f,r11g11b10f_in>",
+       "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f,r11g11b10f_in,srtm_in>"},
+      {"fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8>", "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8,srtm_in>",
+       "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8,r11g11b10f_in>",
+       "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8,r11g11b10f_in,srtm_in>"},
+      {"fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2>", "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2,srtm_in>",
+       "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2,r11g11b10f_in>",
+       "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2,r11g11b10f_in,srtm_in>"}};
+  const int v = (kSrtmIn ? 1 : 0) + (kR11 ? 2 : 0);
+  switch (out_format) {
+    case 1:
+      if constexpr (kR11) fused_r11_quad2x_post_kernel<4, kPostPerSm, __half, kSrtmIn><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      else fused_h_quad2x_post_kernel<4, kPostPerSm, __half, kSrtmIn><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      *name = names[0][v];
       break;
     case 3:
-      fused_h_quad2x_post_kernel<4, kPostPerSm, __half, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
-      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f,srtm_in>";
+      if constexpr (kR11) fused_r11_quad2x_post_kernel<4, kPostPerSm, Unorm8, kSrtmIn><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      else fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm8, kSrtmIn><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      *name = names[1][v];
       break;
-    case 7:
-      fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm8, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
-      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8,srtm_in>";
-      break;
-    case 9:
-      fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm10, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
-      *name = "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2,srtm_in>";
+    case 4:
+      if constexpr (kR11) fused_r11_quad2x_post_kernel<4, kPostPerSm, Unorm10, kSrtmIn><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      else fused_h_quad2x_post_kernel<4, kPostPerSm, Unorm10, kSrtmIn><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, q);
+      *name = names[2][v];
       break;
     default: return cudaErrorNotSupported;
   }
   return cudaGetLastError();
+}
+
+cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const PostParams& q, int out_format, cudaStream_t s,
+                                const char** name, bool srtm_in, bool r11) {
+  if (out_format != 1 && out_format != 3 && out_format != 4) return cudaErrorNotSupported;
+  CUtensorMap tmap;
+  FusedParams p;
+  int per_sm = kPostPerSm;
+  long long grid = 0;
+  const cudaError_t err = fused_setup(e, sharp_h2, out_format == 1 ? 16 : 8, r11, tmap, p, per_sm, grid);
+  if (err != cudaSuccess) return err;
+  if (r11) return srtm_in ? launch_post_kernel<true, true>(p, tmap, q, out_format, grid, s, name)
+                          : launch_post_kernel<false, true>(p, tmap, q, out_format, grid, s, name);
+  return srtm_in ? launch_post_kernel<true, false>(p, tmap, q, out_format, grid, s, name)
+                 : launch_post_kernel<false, false>(p, tmap, q, out_format, grid, s, name);
 }
 #endif
 

@@ -219,7 +219,7 @@ __device__ __forceinline__ void post_pair(const PostParams& q, const PostCursor&
 // launchers (fsr1_fused.cu, fsr1_rcas_packed.cu); out_format 1 RGBA16F, 3 RGBA8_UNORM, 4 RGB10A2_UNORM.  cudaErrorNotSupported: the
 // frame or layout is not one the kernel takes (nothing launched).
 cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const PostParams& q, int out_format, cudaStream_t s,
-                                const char** name, bool srtm_in = false);
+                                const char** name, bool srtm_in = false, bool r11 = false);
 cudaError_t launch_rcas_h_post(const RcasParams& p, const PostParams& q, int out_format, cudaStream_t s, const char** name);
 
 }  // namespace fsr1

@@ -135,10 +135,12 @@ int bpp_of(uint32_t fmt) {
   switch (fmt) {
     case FSR1_FORMAT_RGBA16F: return 8;
     case FSR1_FORMAT_RGBA32F: return 16;
-    case FSR1_FORMAT_RGBA8_UNORM: case FSR1_FORMAT_RGB10A2_UNORM: return 4;
+    case FSR1_FORMAT_RGBA8_UNORM: case FSR1_FORMAT_RGB10A2_UNORM: case FSR1_FORMAT_R11G11B10_FLOAT: return 4;
     default: return 0;
   }
 }
+// the format of EASU's output (the intermediate; the slabs without display steps): RGBA16F for R11G11B10_FLOAT input, an input format only
+uint32_t mid_format(uint32_t fmt) { return fmt == FSR1_FORMAT_R11G11B10_FLOAT ? (uint32_t)FSR1_FORMAT_RGBA16F : fmt; }
 
 struct Rows { uint32_t a, b; };  // [a, b)
 
@@ -321,7 +323,7 @@ fsr1_image make_img(void* data, uint64_t pitch, uint32_t w, uint32_t h, uint32_t
 unsigned char* window_of(const fsr1_shard* s, unsigned char* arena, uint32_t slot) { return arena + kFlagBytes + (uint64_t)slot * s->slot_stride; }
 fsr1_image tmp_of(const fsr1_shard* s, uint32_t slot) {
   return make_img(s->tmp + (uint64_t)slot * s->tmp_slot_stride, s->tmp_pitch, s->out_w, s->out_h, s->easu_rows.a,
-                  s->easu_rows.b - s->easu_rows.a, s->format);
+                  s->easu_rows.b - s->easu_rows.a, mid_format(s->format));
 }
 uint32_t kernel_flags(const fsr1_shard* s) { return (s->flags & ~kShardFlags) | FSR1_FLAG_FUSED; }
 
@@ -366,7 +368,8 @@ extern "C" {
 
 int fsr1_shard_create(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_t out_w, uint32_t out_h, uint32_t format,
                       uint32_t world, uint32_t rank, uint32_t slots, float sharpness_stops, uint32_t flags) {
-  return fsr1_shard_create_post(out_sh, in_w, in_h, out_w, out_h, format, format, nullptr, world, rank, slots, sharpness_stops, flags);
+  return fsr1_shard_create_post(out_sh, in_w, in_h, out_w, out_h, format, mid_format(format), nullptr, world, rank, slots, sharpness_stops,
+                                flags);
 }
 
 int fsr1_shard_create_post(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_t out_w, uint32_t out_h, uint32_t format,
@@ -381,7 +384,7 @@ int fsr1_shard_create_post(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, ui
   if (post_ops) {
     const int rc = fsr1::post_rules(post, format, out_format, flags & ~kShardFlags);
     if (rc != FSR1_OK) return rc;
-  } else if (out_format != format) {
+  } else if (out_format != mid_format(format)) {
     return FSR1_ERR_UNSUPPORTED;
   }
   fsr1_shard* s = new (std::nothrow) fsr1_shard();
@@ -429,7 +432,7 @@ int fsr1_shard_create_post(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, ui
   s->slot_stride = ((uint64_t)s->win_rows_max * s->pitch + 255) & ~(uint64_t)255;
   s->arena_bytes = kFlagBytes + s->slot_stride * slots;
   s->out_pitch = ((uint64_t)out_w * out_bpp + 127) & ~(uint64_t)127;
-  s->tmp_pitch = ((uint64_t)out_w * bpp + 127) & ~(uint64_t)127;  // the intermediate is in the input's format
+  s->tmp_pitch = ((uint64_t)out_w * bpp_of(mid_format(format)) + 127) & ~(uint64_t)127;  // the intermediate: EASU's output format
   s->tmp_slot_stride = (uint64_t)(s->easu_rows.b - s->easu_rows.a) * s->tmp_pitch;
   s->out_slot_stride = (uint64_t)(s->out_rows.b - s->out_rows.a) * s->out_pitch;
   cudaError_t e;

@@ -145,9 +145,10 @@ class _DevBuf:
 
 
 def _tensor_of(img, device):
-    """torch view [rows, width, 4] of an fsr1_image owned by the library ([rows, width] int32 for RGB10A2_UNORM, as api.image takes)."""
+    """torch view [rows, width, 4] of an fsr1_image owned by the library ([rows, width] int32 for RGB10A2_UNORM and R11G11B10_FLOAT, as
+    api.image takes)."""
     import torch
-    if img.format == _lib.FORMAT_RGB10A2_UNORM:
+    if img.format in (_lib.FORMAT_RGB10A2_UNORM, _lib.FORMAT_R11G11B10_FLOAT):
         return torch.as_tensor(_DevBuf(img.data, (img.rows, img.width), (img.pitch_bytes, 4), "<i4"), device=device)
     es, typestr = {_lib.FORMAT_RGBA16F: (2, "<f2"), _lib.FORMAT_RGBA32F: (4, "<f4"), _lib.FORMAT_RGBA8_UNORM: (1, "|u1")}[img.format]
     return torch.as_tensor(_DevBuf(img.data, (img.rows, img.width, 4), (img.pitch_bytes, 4 * es, es), typestr), device=device)
@@ -167,11 +168,13 @@ class ShardedUpscaler:
     (fsr1_shard_create_post), so output(slot) is the display image's rows: uint8 [rows, W, 4] with tepd_bits 8, int32 [rows, W] with 10,
     float16 [rows, W, 4] otherwise.  post(slot, frame=...) describes the next use of a slot (fsr1_shard_post).  The grain / dither
     tiles are device tensors the ranks read while frames are in flight; this object keeps a reference to the ones each slot uses.
+    in_format=FORMAT_R11G11B10_FLOAT (p2p only): the input windows hold R11G11B10_FLOAT codes, int32 [rows, W] (4 B/px: the windows and
+    the halo are half the size of RGBA16F ones); the output slabs are float16 [rows, W, 4] (or the TEPD format).  `dtype` is ignored then.
     """
 
     def __init__(self, in_w, in_h, out_w, out_h, world, rank, sharpness=0.25, dtype=None, device=None, flags=0, slots=1,
                  halo=None, one_stream=False, group=None, skip_halo=False, attach=True, trace=False, dynamic=False,
-                 srtm_inverse=False, grain=None, amount=0.0, tepd_bits=0, dither=None):
+                 srtm_inverse=False, grain=None, amount=0.0, tepd_bits=0, dither=None, in_format=None):
         import torch
         self.rank, self.world, self.slots = int(rank), int(world), int(slots)
         self.in_w, self.in_h, self.out_w, self.out_h = in_w, in_h, out_w, out_h
@@ -192,6 +195,11 @@ class ShardedUpscaler:
             raise ValueError("halo must be 'p2p' or 'nccl'")
         if self.dynamic and halo != "p2p":
             raise ValueError("dynamic=True needs halo='p2p' (the per-frame plan lives in the C ABI's shard)")
+        if in_format not in (None, _lib.FORMAT_R11G11B10_FLOAT):
+            raise ValueError("in_format: None (from dtype) or FORMAT_R11G11B10_FLOAT")
+        if in_format is not None and halo != "p2p":
+            raise ValueError("in_format=FORMAT_R11G11B10_FLOAT needs halo='p2p' (its kernels run inside the C ABI's shard)")
+        self.in_format = in_format
         if self.has_post and halo != "p2p":
             raise ValueError("display steps (srtm_inverse, grain, tepd_bits) need halo='p2p' (they run inside the C ABI's shard)")
         self.halo_mode = halo
@@ -207,10 +215,14 @@ class ShardedUpscaler:
     def _init_p2p(self, sharpness, dtype, one_stream, skip_halo=False, attach=True, trace=False):
         import torch
         L = _lib.lib()
-        fmt = {torch.float16: _lib.FORMAT_RGBA16F, torch.float32: _lib.FORMAT_RGBA32F, torch.uint8: _lib.FORMAT_RGBA8_UNORM}[dtype]
+        if self.in_format is not None:
+            fmt = self.in_format
+        else:
+            fmt = {torch.float16: _lib.FORMAT_RGBA16F, torch.float32: _lib.FORMAT_RGBA32F, torch.uint8: _lib.FORMAT_RGBA8_UNORM}[dtype]
         srtm_inverse, grain, amount, tepd_bits, dither = self._post_args
         post, keep = api._post(srtm_inverse, grain, amount, tepd_bits, dither, 0)
-        out_fmt = {0: fmt, 8: _lib.FORMAT_RGBA8_UNORM, 10: _lib.FORMAT_RGB10A2_UNORM}[tepd_bits]
+        mid_fmt = _lib.FORMAT_RGBA16F if fmt == _lib.FORMAT_R11G11B10_FLOAT else fmt   # EASU's output format
+        out_fmt = {0: mid_fmt, 8: _lib.FORMAT_RGBA8_UNORM, 10: _lib.FORMAT_RGB10A2_UNORM}[tepd_bits]
         self._tiles = [(grain, dither)] * self.slots     # the tiles each slot's next use reads
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):

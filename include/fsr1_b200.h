@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame, fsr1_shard_create_post / fsr1_shard_post */
+#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame, fsr1_shard_create_post / fsr1_shard_post, FSR1_FORMAT_R11G11B10_FLOAT */
 
 enum {
   FSR1_OK = 0,
@@ -59,7 +59,19 @@ enum {
   FSR1_FORMAT_RGBA16F = 1,
   FSR1_FORMAT_RGBA32F = 2,
   FSR1_FORMAT_RGBA8_UNORM = 3,    /* 4 B/px, byte order R,G,B,A (DXGI_FORMAT_R8G8B8A8_UNORM)                      */
-  FSR1_FORMAT_RGB10A2_UNORM = 4   /* 4 B/px, bits 0-9 R, 10-19 G, 20-29 B, 30-31 A (DXGI_FORMAT_R10G10B10A2_UNORM) */
+  FSR1_FORMAT_RGB10A2_UNORM = 4,  /* 4 B/px, bits 0-9 R, 10-19 G, 20-29 B, 30-31 A (DXGI_FORMAT_R10G10B10A2_UNORM) */
+  FSR1_FORMAT_R11G11B10_FLOAT = 5 /* 4 B/px, unsigned floats (DXGI_FORMAT_R11G11B10_FLOAT): bits 0-10 R and 11-21 G, each 6 mantissa
+                                     bits below 5 exponent bits; bits 22-31 B, 5 mantissa bits below 5 exponent bits; exponent bias 15,
+                                     no alpha.  An INPUT format only: every channel is a half without its sign and low mantissa bits,
+                                     so the kernels decode each texel exactly to the RGBA16F texel (R, G, B, 1.0) as they load it
+                                     (denormals, inf and NaN included), and every call is bit-identical to the same call on that RGBA16F
+                                     image of the decoded values.  Where it is the input, EASU's output, the intermediate and the output
+                                     are RGBA16F (with fsr1_upscale_post's TEPD, the UNORM format TEPD implies).  fsr1_easu,
+                                     fsr1_upscale*, fsr1_context_* and fsr1_shard_* take it, on the RGBA16F kernels (tiled, fused, post,
+                                     with FSR1_FLAG_SRTM_INPUT too) and, for the layouts, scales and FSR1_FLAG_FORCE_DIRECT those decline,
+                                     the fp32 direct kernel.  FSR1_ERR_UNSUPPORTED, before any CUDA call: as any output, as RCAS input,
+                                     as an image or tile of the pointwise passes, and combined with FSR1_FLAG_EXACT / H_REFERENCE /
+                                     PRECISE / RCAS_HX2. */
 };
 
 enum {
@@ -93,7 +105,7 @@ enum {
                                        after RCAS with fsr1_upscale_post's FSR1_POST_SRTM_INVERSE: the full HDR round trip.
                                        fsr1_easu, fsr1_upscale*, fsr1_context_* and fsr1_shard_* take it (RCAS never sees it; the shard's
                                        halo carries raw input rows and fsr1_easu_input_rows is unchanged: SRTM is pointwise).  RGBA16F
-                                       input on the TMA-tiled kernels only: FSR1_ERR_UNSUPPORTED, with nothing launched, for another input
+                                       (or R11G11B10_FLOAT, decoded first) input on the TMA-tiled kernels only: FSR1_ERR_UNSUPPORTED, with nothing launched, for another input
                                        format, EXACT / FORCE_DIRECT / H_REFERENCE / PRECISE, an input (or EASU output) whose base or pitch
                                        is not 16-byte aligned, or constants that do not upscale (0 < con0.x, con0.y <= 1).
                                        fsr1_rcas: FSR1_ERR_INVALID_ARGUMENT. */
@@ -116,7 +128,8 @@ typedef struct fsr1_image {
   uint32_t reserved;
 } fsr1_image;
 
-/* EASU over output rows [y0, y1) (y1 == 0 means "to the last row").  con = con0..con3, 16 words. */
+/* EASU over output rows [y0, y1) (y1 == 0 means "to the last row").  con = con0..con3, 16 words.  in and out have the same format, but
+ * for R11G11B10_FLOAT input, whose output is RGBA16F. */
 int fsr1_easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], uint32_t y0, uint32_t y1,
               uint32_t flags, void* stream);
 
@@ -129,7 +142,8 @@ int fsr1_rcas(const fsr1_image* in, const fsr1_image* out, const uint32_t con[4]
 int fsr1_easu_input_rows(const uint32_t con[16], uint32_t in_height, uint32_t y0, uint32_t y1,
                          uint32_t* first_row, uint32_t* last_row);
 
-/* EASU -> RCAS for output rows [y0,y1).  `tmp` is the display-sized intermediate (same format as out);
+/* EASU -> RCAS for output rows [y0,y1).  `tmp` is the display-sized intermediate (same format as out; both RGBA16F for
+ * R11G11B10_FLOAT input);
  * it must hold rows [y0-1, y1+1) clipped to the image.  easu_con 16 words, rcas_con 4 words. */
 int fsr1_upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, const uint32_t easu_con[16],
                  const uint32_t rcas_con[4], uint32_t y0, uint32_t y1, uint32_t flags, void* stream);
@@ -137,7 +151,8 @@ int fsr1_upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
 /* ---- resource-owning context (the FSR_Filter object of the sample) ---------------------------- */
 typedef struct fsr1_context fsr1_context;
 
-/* Allocates the intermediate image for (out_width x out_height, format) on the current device. */
+/* Allocates the intermediate image for (out_width x out_height, format) on the current device.  `format` is the input's; the
+ * intermediate and the output are in that format too, but RGBA16F for R11G11B10_FLOAT. */
 int fsr1_context_create(fsr1_context** ctx, uint32_t in_width, uint32_t in_height, uint32_t out_width,
                         uint32_t out_height, uint32_t format);
 void fsr1_context_destroy(fsr1_context* ctx);
@@ -273,7 +288,7 @@ int fsr1_tepd_h(const fsr1_image* in, const fsr1_image* dither, const fsr1_image
  *     FSR1_POST_LFGA:          fsr1_lfga(T, grain, T, lfga_amount, ...) FsrLfgaF        ffx_fsr1.h:1014
  *     FSR1_POST_TEPD8 / 10:    fsr1_tepd(T, dither, out, 8 / 10, frame, ...)  FsrTepdC8F / C10F  ffx_fsr1.h:1100-1126
  * in that order (the last step writes `out`).  Alpha is what RCAS stores (1, or the input's with FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA).
- *   in      RGBA16F.
+ *   in      RGBA16F or R11G11B10_FLOAT.
  *   out     RGBA16F; with TEPD also RGBA8_UNORM (TEPD8) or RGB10A2_UNORM (TEPD10): the code values, as fsr1_tepd writes them.
  *   tmp     the RGBA16F intermediate of the two-kernel path (as fsr1_upscale); NULL is accepted when the frame takes the fused
  *           kernel (FSR1_FLAG_FUSED, exactly 2x, no RCAS option, no OUTPUT_SQUARE, no PRECISE), which then is the only launch.
@@ -295,7 +310,7 @@ typedef struct fsr1_post {
 int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, const uint32_t easu_con[16],
                       const uint32_t rcas_con[4], const fsr1_post* post, uint32_t y0, uint32_t y1, uint32_t flags, void* stream);
 /* The context form, as fsr1_context_upscale_render (render size 0 = the context's input size; always FSR1_FLAG_FUSED).  The context's
- * format must be RGBA16F.  `out_dev` is RGBA8_UNORM with TEPD8, RGB10A2_UNORM with TEPD10, RGBA16F otherwise. */
+ * format must be RGBA16F or R11G11B10_FLOAT.  `out_dev` is RGBA8_UNORM with TEPD8, RGB10A2_UNORM with TEPD10, RGBA16F otherwise. */
 int fsr1_context_upscale_post(fsr1_context* ctx, const void* in_dev, uint64_t in_pitch, uint32_t render_width,
                               uint32_t render_height, void* out_dev, uint64_t out_pitch, float sharpness_stops,
                               const fsr1_post* post, uint32_t flags, void* stream);
@@ -304,9 +319,11 @@ int fsr1_context_upscale_post(fsr1_context* ctx, const void* in_dev, uint64_t in
  * so each rank's output slab holds the display image's rows (for rows [out_row0, out_row1), bit-identical to the same rows of
  * fsr1_upscale_post / fsr1_context_upscale_post on the whole frame) and no pass runs over the slabs afterwards.  fsr1_shard_create is
  * fsr1_shard_create_post(..., format, format, NULL, ...).
- *   format      the input's format; with post ops RGBA16F only.
+ *   format      the input's format; with post ops RGBA16F or R11G11B10_FLOAT.  The windows and the halo are sized at its bytes per
+ *               pixel (4 for R11G11B10_FLOAT); an intermediate, when there is one, is in EASU's output format (RGBA16F for it).
  *   out_format  the slabs' format: RGBA16F, or with TEPD the UNORM format it implies (RGBA8_UNORM for TEPD8, RGB10A2_UNORM for
- *               TEPD10, 4 B/px); without post ops it must equal `format`.  fsr1_shard_output describes slabs in this format.
+ *               TEPD10, 4 B/px); without post ops it must equal `format`, but RGBA16F for R11G11B10_FLOAT input (fsr1_shard_create
+ *               gives RGBA16F slabs then).  fsr1_shard_output describes slabs in this format.
  *   post        NULL or ops == 0: no display steps.  `post->ops` is fixed for the shard's life (it decides which kernels the create-time
  *               dry frames load); the rest is the first description of every slot (fsr1_shard_post).  The tiles (grain, dither) are
  *               whole device images on the rank's own device, read by every frame that uses them: the caller keeps them alive and
