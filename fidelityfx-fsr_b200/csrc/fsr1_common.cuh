@@ -4,8 +4,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
+#include <string.h>
 
-struct fsr1_post;  // include/fsr1_b200.h
+#include "../../include/fsr1_b200.h"
 
 namespace fsr1 {
 
@@ -45,6 +46,14 @@ struct EasuParams {
   int y0, y1;                // output rows [y0,y1)
   HaloSync sync = {};
 };
+
+// The two tests of the EASU constants every kernel choice depends on (con0 of FsrEasuCon: scale.xy, offset.zw): exactly 2x (the 2x
+// kernels) and upscaling (the any-scale tiled kernels).  They are also the kinds of frame a dynamic fsr1_shard loads kernels for at
+// create (frame_kind, fsr1_shard.cu), so a kernel choice on any other property of the constants needs a kind of its own there.
+__host__ __device__ inline bool is_2x(float c0x, float c0y, float c0z, float c0w) {
+  return c0x == 0.5f && c0y == 0.5f && c0z == -0.25f && c0w == -0.25f;
+}
+__host__ __device__ inline bool is_upscale(float c0x, float c0y) { return c0x > 0.0f && c0x <= 1.0f && c0y > 0.0f && c0y <= 1.0f; }
 
 struct RcasParams {
   ImgView in, out;
@@ -255,14 +264,39 @@ __device__ __forceinline__ void halo_sync_end(const HaloSync& hs) {
 
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(max(v, lo), hi); }
 
+// ---- host helpers of the dispatch layer (fsr1_capi.cu, fsr1_shard.cu) -----------------------------------------------------
+inline int bytes_per_pixel(uint32_t fmt) {  // 0: not a format include/fsr1_b200.h defines
+  switch (fmt) {
+    case FSR1_FORMAT_RGBA16F: return 8;
+    case FSR1_FORMAT_RGBA32F: return 16;
+    case FSR1_FORMAT_RGBA8_UNORM: case FSR1_FORMAT_RGB10A2_UNORM: case FSR1_FORMAT_R11G11B10_FLOAT: return 4;
+    default: return 0;
+  }
+}
+// The format of the image EASU writes from an input of format `fmt`: R11G11B10_FLOAT is an input format only, its EASU output (and
+// every intermediate and output after it) is RGBA16F, the exact superset of its values.
+inline uint32_t easu_out_format(uint32_t fmt) { return fmt == FSR1_FORMAT_R11G11B10_FLOAT ? (uint32_t)FSR1_FORMAT_RGBA16F : fmt; }
+inline float word_as_float(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }  // a constant word of FsrEasuCon / FsrRcasCon
+struct Rows { uint32_t a, b; };  // [a, b)
+// The rows EASU writes for output rows [y0, y1) of an image out_h rows tall, and the rows RCAS reads for them: one more on each side
+// inside the image.  So a row slab's EASU produces the apron its RCAS reads, and needs no second exchange.
+inline Rows easu_rows(uint32_t y0, uint32_t y1, uint32_t out_h) { return Rows{y0 == 0 ? 0 : y0 - 1, y1 >= out_h ? out_h : y1 + 1}; }
+
 void set_last_detail(int v);  // fsr1_capi.cu: detail word reported by fsr1_last_cuda_error()
-// fsr1_shard.cu -> fsr1_capi.cu: the hand-shake the NEXT EASU (or fused) launch on this thread should carry; consumed() tells whether the
-// kernel that was launched took it (the TMA-tiled fp16 kernels do; otherwise the shard falls back to its own tiny wait / signal kernels)
-void set_halo_sync(const HaloSync* hs);
-bool halo_sync_consumed();
 // fsr1_capi.cu -> fsr1_shard.cu: the rules fsr1_upscale_post applies to the post description (ops, tiles), the formats and the flags,
 // with the error it would return; no CUDA call.  The frame's images (sizes, windows, alignment) are checked by each launch.
 int post_rules(const ::fsr1_post* post, uint32_t in_format, uint32_t out_format, uint32_t flags);
+// fsr1_capi.cu -> fsr1_shard.cu: fsr1_easu, fsr1_upscale and fsr1_upscale_post (which call them with nulls) for a frame of a sharded
+// stream.  `sync`: the neighbour hand-shake the EASU (or fused) kernel is to carry; null outside the sharded path.  *sync_taken is set
+// to true when a kernel that carries it launched (the TMA-tiled fp16 and the fused kernels do), and left alone otherwise: the shard
+// then runs its own tiny wait / signal kernels around the frame.  sync_taken may be null when sync is.
+int easu(const ::fsr1_image* in, const ::fsr1_image* out, const uint32_t con[16], uint32_t y0, uint32_t y1, uint32_t flags, void* stream,
+         const HaloSync* sync, bool* sync_taken);
+int upscale(const ::fsr1_image* in, const ::fsr1_image* tmp, const ::fsr1_image* out, const uint32_t easu_con[16],
+            const uint32_t rcas_con[4], uint32_t y0, uint32_t y1, uint32_t flags, void* stream, const HaloSync* sync, bool* sync_taken);
+int upscale_post(const ::fsr1_image* in, const ::fsr1_image* tmp, const ::fsr1_image* out, const uint32_t easu_con[16],
+                 const uint32_t rcas_con[4], const ::fsr1_post* post, uint32_t y0, uint32_t y1, uint32_t flags, void* stream,
+                 const HaloSync* sync, bool* sync_taken);
 
 // launchers (defined in the .cu files, called from fsr1_capi.cu)
 cudaError_t launch_easu_direct(const EasuParams& p, int format, bool exact, cudaStream_t s, const char** name);

@@ -437,7 +437,7 @@ static cudaError_t launch_pairs_f32math(const EasuParams& p, cudaStream_t s, con
   constexpr int kB = Tex<S>::kBytes;
   if ((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15) || (reinterpret_cast<uintptr_t>(p.out.base) & 15) || (p.out.pitch & 15))
     return cudaErrorNotSupported;
-  if (!(p.c0x > 0.0f && p.c0x <= 1.0f && p.c0y > 0.0f && p.c0y <= 1.0f)) return cudaErrorNotSupported;  // upscaling only
+  if (!is_upscale(p.c0x, p.c0y)) return cudaErrorNotSupported;
   EncodeTiledFn encode = get_encode_fn();
   if (!encode) return cudaErrorNotSupported;
   int BW = f_max_footprint(p.out.w, 0, kFTileW, p.c0x, p.c0z, kB == 8);
@@ -481,7 +481,7 @@ static cudaError_t launch_quad_f32math(const EasuParams& p, cudaStream_t s, cons
   if ((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15) || (reinterpret_cast<uintptr_t>(p.out.base) & 15) ||
       (p.out.pitch & 15))
     return cudaErrorNotSupported;
-  if (!(p.c0x == 0.5f && p.c0y == 0.5f && p.c0z == -0.25f && p.c0w == -0.25f)) return cudaErrorNotSupported;  // 2x only
+  if (!is_2x(p.c0x, p.c0y, p.c0z, p.c0w)) return cudaErrorNotSupported;
   EncodeTiledFn encode = get_encode_fn();
   if (!encode) return cudaErrorNotSupported;
   constexpr int NW = 4, per_sm = 4;

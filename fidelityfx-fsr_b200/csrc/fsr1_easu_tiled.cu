@@ -499,10 +499,6 @@ static int max_footprint(int n_out, int first, int tile, float scale, float offs
   return best;
 }
 
-// The scale tests of the launchers (this one, "upscaling only", and fused_setup's) are the kinds of frame a dynamic fsr1_shard
-// loads kernels for at create (frame_kind, fsr1_shard.cu): keep the two in step.
-static bool is_2x(const EasuParams& p) { return p.c0x == 0.5f && p.c0y == 0.5f && p.c0z == -0.25f && p.c0w == -0.25f; }
-
 // tiles of the 2x kernels: cells k in [-1, k_last], rows of cells from the one holding output row y0
 struct QuadGrid { int tiles_x, n_tiles, m_first, grid; };
 static QuadGrid quad_grid(const EasuParams& p, int cy, int ctas_per_sm) {
@@ -520,7 +516,7 @@ static QuadGrid quad_grid(const EasuParams& p, int cy, int ctas_per_sm) {
 // 2-4 code values off where the 8-bit format is within one; the caller also routes FSR1_FLAG_PRECISE / _EXACT there.)
 cudaError_t launch_easu_u_tiled(const EasuParams& p, int format, cudaStream_t s, const char** name) {
   if (format != 3) return cudaErrorNotSupported;
-  if ((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15) || !is_2x(p)) return cudaErrorNotSupported;  // TMA
+  if ((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15) || !is_2x(p.c0x, p.c0y, p.c0z, p.c0w)) return cudaErrorNotSupported;  // TMA
   constexpr int NW = 4, CY = 2 * NW;
   CUtensorMap tmap;
   if (!make_tmap(&tmap, p.in, kUBW, CY + 3, CU_TENSOR_MAP_DATA_TYPE_UINT32)) return cudaErrorNotSupported;
@@ -538,7 +534,7 @@ cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char*
   CUtensorMap tmap;
   const CUtensorMapDataType type = r11 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT64;
 
-  if (is_2x(p)) {
+  if (is_2x(p.c0x, p.c0y, p.c0z, p.c0w)) {
     // 4 warps x 7 CTAs per SM: the kernel needs 72 registers, exactly what 7 x 128 threads allow.  A launch that waits
     // for a neighbour's halo (p.sync, fsr1_shard.cu) is capped at 6 CTAs per SM: at 7 every warp scheduler's 16384
     // registers are taken but 256, so the one-warp halo_push_kernel that the wait depends on cannot be placed beside a
@@ -562,7 +558,7 @@ cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char*
     return cudaGetLastError();
   }
 
-  if (!(p.c0x > 0.0f && p.c0x <= 1.0f && p.c0y > 0.0f && p.c0y <= 1.0f)) return cudaErrorNotSupported;  // upscaling only
+  if (!is_upscale(p.c0x, p.c0y)) return cudaErrorNotSupported;
   int BW = max_footprint(p.out.w, 0, kTileW, p.c0x, p.c0z, true);
   int BH = max_footprint(p.y1, p.y0, kTileH, p.c0y, p.c0w, false);
   BW = (BW + 1) & ~1;  // inner box extent must be a multiple of 16 bytes

@@ -340,7 +340,7 @@ fused_r11_quad2x_post_kernel(const FusedParams p, const __grid_constant__ CUtens
 // out_align: the alignment the output store needs (16 for RGBA16F pairs, 8 for UNORM pairs).
 static cudaError_t fused_setup(const EasuParams& e, uint32_t sharp_h2, int out_align, bool r11, CUtensorMap& tmap, FusedParams& p,
                                int& per_sm, long long& grid) {
-  if (!(e.c0x == 0.5f && e.c0y == 0.5f && e.c0z == -0.25f && e.c0w == -0.25f)) return cudaErrorNotSupported;
+  if (!is_2x(e.c0x, e.c0y, e.c0z, e.c0w)) return cudaErrorNotSupported;
   if ((reinterpret_cast<uintptr_t>(e.in.base) & 15) || (e.in.pitch & 15) || (reinterpret_cast<uintptr_t>(e.out.base) & (out_align - 1)) ||
       (e.out.pitch & (out_align - 1)))
     return cudaErrorNotSupported;

@@ -55,6 +55,9 @@
 
 namespace {
 
+using fsr1::bytes_per_pixel;
+using fsr1::easu_out_format;
+using fsr1::Rows;
 using fsr1::spin_until;
 using fsr1::st_release_sys;
 
@@ -131,28 +134,15 @@ __global__ void __launch_bounds__(32) credit_signal_kernel(uint32_t* credit_up, 
   if (f) st_release_sys(f, q);
 }
 
-int bpp_of(uint32_t fmt) {
-  switch (fmt) {
-    case FSR1_FORMAT_RGBA16F: return 8;
-    case FSR1_FORMAT_RGBA32F: return 16;
-    case FSR1_FORMAT_RGBA8_UNORM: case FSR1_FORMAT_RGB10A2_UNORM: case FSR1_FORMAT_R11G11B10_FLOAT: return 4;
-    default: return 0;
-  }
-}
-// the format of EASU's output (the intermediate; the slabs without display steps): RGBA16F for R11G11B10_FLOAT input, an input format only
-uint32_t mid_format(uint32_t fmt) { return fmt == FSR1_FORMAT_R11G11B10_FLOAT ? (uint32_t)FSR1_FORMAT_RGBA16F : fmt; }
-
-struct Rows { uint32_t a, b; };  // [a, b)
-
 // the fsr1_shard_* bits of the create flags; the rest are FSR1_FLAG_* for the kernels
 constexpr uint32_t kShardFlags = FSR1_SHARD_ONE_STREAM | FSR1_SHARD_SKIP_HALO | FSR1_SHARD_TRACE | FSR1_SHARD_DYNAMIC;
 
 // Kinds of frame that fsr1_upscale may run on different kernels: exactly 2x (the fused / 2x-tiled kernels), any other upscale
 // (the any-scale tiled kernels), and everything else (direct kernels).  Whether the EASU kernel carries the halo hand-shake
 // itself is a property of the kind: RGBA16F upscales (2x and any scale) take launch_easu_h_tiled / the fused kernel, which do;
-// RGBA16F downscales, FSR1_FLAG_PRECISE, fp32 and UNORM frames take kernels that do not.  The kinds mirror the dispatch rules of
-// fsr1_upscale / fsr1_easu (is_2x and "upscaling only" in the launchers): a launcher that chose between kernels WITHIN a kind
-// would have to become a kind of its own here, or its second kernel would be loaded lazily while flag-waiting kernels spin.
+// RGBA16F downscales, FSR1_FLAG_PRECISE, fp32 and UNORM frames take kernels that do not.  The kinds are the two scale tests every
+// launcher chooses by (is_2x, is_upscale, fsr1_common.cuh): a launcher that chose between kernels WITHIN a kind would have to become
+// a kind of its own here, or its second kernel would be loaded lazily while flag-waiting kernels spin.
 enum { kFrame2x = 0, kFrameUp = 1, kFrameOther = 2, kFrameKinds = 3 };
 
 // One use of a slot: render size, constants, and this rank's rows for it (fsr1_shard_frame; the create-time frame otherwise).
@@ -212,7 +202,7 @@ Rows plan_out_rows(const fsr1_shard* s, uint32_t r) {
 }
 Rows plan_easu_rows(const fsr1_shard* s, uint32_t r) {
   const Rows o = plan_out_rows(s, r);
-  return Rows{o.a == 0 ? 0 : o.a - 1, o.b >= s->out_h ? s->out_h : o.b + 1};
+  return fsr1::easu_rows(o.a, o.b, s->out_h);
 }
 // input rows of a frame `rh` rows tall
 Rows plan_owned(const fsr1_shard* s, uint32_t rh, uint32_t r) {
@@ -229,12 +219,11 @@ Rows plan_window(const fsr1_shard* s, const uint32_t econ[16], uint32_t rh, uint
   return Rows{o.a < n.a ? o.a : n.a, o.b > n.b ? o.b : n.b};
 }
 
-float word_as_float(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
-
 int frame_kind(const uint32_t econ[16]) {
-  const float sx = word_as_float(econ[0]), sy = word_as_float(econ[1]);
-  if (sx == 0.5f && sy == 0.5f && word_as_float(econ[2]) == -0.25f && word_as_float(econ[3]) == -0.25f) return kFrame2x;
-  return sx > 0.0f && sx <= 1.0f && sy > 0.0f && sy <= 1.0f ? kFrameUp : kFrameOther;
+  const float c0x = fsr1::word_as_float(econ[0]), c0y = fsr1::word_as_float(econ[1]), c0z = fsr1::word_as_float(econ[2]),
+              c0w = fsr1::word_as_float(econ[3]);
+  if (fsr1::is_2x(c0x, c0y, c0z, c0w)) return kFrame2x;
+  return fsr1::is_upscale(c0x, c0y) ? kFrameUp : kFrameOther;
 }
 
 // The plan of frame rw x rh for this rank, with the constants context_run builds (FsrEasuCon(rw, rh, rw, rh, out_w, out_h),
@@ -323,7 +312,7 @@ fsr1_image make_img(void* data, uint64_t pitch, uint32_t w, uint32_t h, uint32_t
 unsigned char* window_of(const fsr1_shard* s, unsigned char* arena, uint32_t slot) { return arena + kFlagBytes + (uint64_t)slot * s->slot_stride; }
 fsr1_image tmp_of(const fsr1_shard* s, uint32_t slot) {
   return make_img(s->tmp + (uint64_t)slot * s->tmp_slot_stride, s->tmp_pitch, s->out_w, s->out_h, s->easu_rows.a,
-                  s->easu_rows.b - s->easu_rows.a, mid_format(s->format));
+                  s->easu_rows.b - s->easu_rows.a, easu_out_format(s->format));
 }
 uint32_t kernel_flags(const fsr1_shard* s) { return (s->flags & ~kShardFlags) | FSR1_FLAG_FUSED; }
 
@@ -337,8 +326,9 @@ void set_slot_post(fsr1_shard* s, uint32_t slot, const fsr1_post* post) {
   if (d.has_dither) d.dither = *post->dither;
 }
 
-// The frame described by slot `slot` (its plan and post) on stream `st`: fsr1_upscale_post, which is fsr1_upscale without post ops.
-int launch_frame(fsr1_shard* s, uint32_t slot, cudaStream_t st) {
+// The frame described by slot `slot` (its plan and post) on stream `st`: fsr1_upscale_post, which is fsr1_upscale without post ops,
+// with the neighbour hand-shake `sync` (fsr1::upscale_post).
+int launch_frame(fsr1_shard* s, uint32_t slot, cudaStream_t st, const fsr1::HaloSync* sync, bool* sync_taken) {
   const FramePlan& p = s->plan[slot];
   fsr1_image win, out, tmp;
   fsr1_shard_window(s, slot, &win);
@@ -346,8 +336,8 @@ int launch_frame(fsr1_shard* s, uint32_t slot, cudaStream_t st) {
   if (s->tmp) tmp = tmp_of(s, slot);
   const SlotPost& d = s->post[slot];
   const fsr1_post post = {s->post_ops, d.lfga_amount, d.has_grain ? &d.grain : nullptr, d.has_dither ? &d.dither : nullptr, d.frame, 0};
-  return fsr1_upscale_post(&win, s->tmp ? &tmp : nullptr, &out, p.econ, p.rcon, s->post_ops ? &post : nullptr, s->out_rows.a,
-                           s->out_rows.b, kernel_flags(s), st);
+  return fsr1::upscale_post(&win, s->tmp ? &tmp : nullptr, &out, p.econ, p.rcon, s->post_ops ? &post : nullptr, s->out_rows.a,
+                            s->out_rows.b, kernel_flags(s), st, sync, sync_taken);
 }
 
 // One dry frame `p` on the zero-filled slot 0 (no halo protocol), through the intermediate if there is one: loads the kernels
@@ -355,11 +345,8 @@ int launch_frame(fsr1_shard* s, uint32_t slot, cudaStream_t st) {
 int dry_frame(fsr1_shard* s, const FramePlan& p, bool* inkernel) {
   s->plan[0] = p;
   const fsr1::HaloSync none = {};
-  fsr1::set_halo_sync(&none);
-  const int rc = launch_frame(s, 0, s->s_easu);
-  *inkernel = fsr1::halo_sync_consumed();
-  fsr1::set_halo_sync(nullptr);
-  return rc;
+  *inkernel = false;
+  return launch_frame(s, 0, s->s_easu, &none, inkernel);
 }
 
 }  // namespace
@@ -368,7 +355,7 @@ extern "C" {
 
 int fsr1_shard_create(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, uint32_t out_w, uint32_t out_h, uint32_t format,
                       uint32_t world, uint32_t rank, uint32_t slots, float sharpness_stops, uint32_t flags) {
-  return fsr1_shard_create_post(out_sh, in_w, in_h, out_w, out_h, format, mid_format(format), nullptr, world, rank, slots, sharpness_stops,
+  return fsr1_shard_create_post(out_sh, in_w, in_h, out_w, out_h, format, easu_out_format(format), nullptr, world, rank, slots, sharpness_stops,
                                 flags);
 }
 
@@ -376,7 +363,7 @@ int fsr1_shard_create_post(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, ui
                            uint32_t out_format, const fsr1_post* post, uint32_t world, uint32_t rank, uint32_t slots, float sharpness_stops,
                            uint32_t flags) {
   if (!out_sh || !in_w || !in_h || !out_w || !out_h || !world || rank >= world || !slots || slots > kMaxSlots) return FSR1_ERR_INVALID_ARGUMENT;
-  const int bpp = bpp_of(format), out_bpp = bpp_of(out_format);
+  const int bpp = bytes_per_pixel(format), out_bpp = bytes_per_pixel(out_format);
   if (!bpp || !out_bpp) return FSR1_ERR_INVALID_ARGUMENT;
   if (world > in_h || world > out_h) return FSR1_ERR_INVALID_ARGUMENT;  // no empty slabs
   // the display steps: fsr1_upscale_post's rules, before any CUDA call; without them the slabs are in the input's format
@@ -384,7 +371,7 @@ int fsr1_shard_create_post(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, ui
   if (post_ops) {
     const int rc = fsr1::post_rules(post, format, out_format, flags & ~kShardFlags);
     if (rc != FSR1_OK) return rc;
-  } else if (out_format != mid_format(format)) {
+  } else if (out_format != easu_out_format(format)) {
     return FSR1_ERR_UNSUPPORTED;
   }
   fsr1_shard* s = new (std::nothrow) fsr1_shard();
@@ -432,7 +419,7 @@ int fsr1_shard_create_post(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, ui
   s->slot_stride = ((uint64_t)s->win_rows_max * s->pitch + 255) & ~(uint64_t)255;
   s->arena_bytes = kFlagBytes + s->slot_stride * slots;
   s->out_pitch = ((uint64_t)out_w * out_bpp + 127) & ~(uint64_t)127;
-  s->tmp_pitch = ((uint64_t)out_w * bpp_of(mid_format(format)) + 127) & ~(uint64_t)127;  // the intermediate: EASU's output format
+  s->tmp_pitch = ((uint64_t)out_w * bytes_per_pixel(easu_out_format(format)) + 127) & ~(uint64_t)127;  // the intermediate: EASU's output format
   s->tmp_slot_stride = (uint64_t)(s->easu_rows.b - s->easu_rows.a) * s->tmp_pitch;
   s->out_slot_stride = (uint64_t)(s->out_rows.b - s->out_rows.a) * s->out_pitch;
   cudaError_t e;
@@ -546,7 +533,7 @@ int fsr1_shard_geometry(const fsr1_shard* s, fsr1_shard_info* info) {
   info->window_row0 = p.window.a; info->window_row1 = p.window.b;
   info->send_up_row0 = p.send[kFromUp].a; info->send_up_row1 = p.send[kFromUp].b;
   info->send_down_row0 = p.send[kFromDown].a; info->send_down_row1 = p.send[kFromDown].b;
-  info->halo_recv_bytes = (uint64_t)((p.owned.a - p.window.a) + (p.window.b - p.owned.b)) * s->in_w * bpp_of(s->format);
+  info->halo_recv_bytes = (uint64_t)((p.owned.a - p.window.a) + (p.window.b - p.owned.b)) * s->in_w * bytes_per_pixel(s->format);
   info->arena_bytes = s->arena_bytes;
   return FSR1_OK;
 }
@@ -711,10 +698,8 @@ int fsr1_shard_submit(fsr1_shard* s, uint32_t slot, void* stream) {
     halo_wait_kernel<<<1, 32, 0, sk>>>(hs.ready[kFromUp], hs.ready[kFromDown], q, flags + kStatusIdx);
     if ((e = cudaGetLastError()) != cudaSuccess) return cuda_rc(e);
   }
-  if (inkernel) fsr1::set_halo_sync(&hs);
-  int rc = launch_frame(s, slot, sk);
-  const bool took = inkernel && fsr1::halo_sync_consumed();
-  fsr1::set_halo_sync(nullptr);
+  bool took = false;
+  const int rc = launch_frame(s, slot, sk, inkernel ? &hs : nullptr, &took);
   if (rc != FSR1_OK) return rc;
   if (inkernel && !took) return FSR1_ERR_UNSUPPORTED;  // cannot happen: the capability was probed with this configuration
   if (shake && !inkernel) {

@@ -36,7 +36,7 @@ def frame(w, h):
 
 def exactly_2x(iw, ih):
     """FsrEasuCon computes in * rcp(out) in fp32: for some sizes 'twice' is 0.49999997, and the launchers then take the any-scale
-    kernel (is_2x() in csrc/fsr1_easu_tiled.cu, the same test in fsr1_fused.cu); the campaign follows them."""
+    kernel (is_2x() in csrc/fsr1_common.cuh); the campaign follows them."""
     return ol.easu_con(iw, ih, 2 * iw, 2 * ih)[:4] == [0x3f000000, 0x3f000000, 0xbe800000, 0xbe800000]
 
 
