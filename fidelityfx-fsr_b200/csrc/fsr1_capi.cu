@@ -84,7 +84,64 @@ int host_cell(uint32_t o, float scale, float offset) {
 constexpr uint32_t kAllFlags = FSR1_FLAG_RCAS_CLAMP | FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_NO_RCAS |
                                FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_DENOISE |
                                FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA | FSR1_FLAG_OUTPUT_SQUARE | FSR1_FLAG_FUSED | FSR1_FLAG_RCAS_HX2 |
-                               FSR1_FLAG_SRTM_INPUT;
+                               FSR1_FLAG_SRTM_INPUT | FSR1_FLAG_IN_SURFACE | FSR1_FLAG_OUT_SURFACE;
+
+// ---- surface images (FSR1_FLAG_IN_SURFACE / FSR1_FLAG_OUT_SURFACE, include/fsr1_b200.h) ------------------------------------------
+constexpr uint32_t kSurfFlags = FSR1_FLAG_IN_SURFACE | FSR1_FLAG_OUT_SURFACE;
+// the surface stages exist in the RGBA16F production kernels only (tiled EASU, packed RCAS, fused, post)
+constexpr uint32_t kSurfRefused = FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_HX2;
+
+// The layout of a surface image: a handle, pitch 0, the whole image (never a window).  No CUDA call.
+int check_surface(const fsr1_image* im) {
+  if (!im || !im->data || im->width == 0 || im->height == 0 || im->width > 32768u || im->height > 32768u) return FSR1_ERR_INVALID_ARGUMENT;
+  if (!bytes_per_pixel(im->format) || im->pitch_bytes != 0 || im->row0 != 0 || im->rows != im->height) return FSR1_ERR_INVALID_ARGUMENT;
+  return FSR1_OK;
+}
+// an image the call reads or writes: a surface image when the flag that describes it is set, a linear one otherwise
+int check_io(const fsr1_image* im, bool surface) { return surface ? check_surface(im) : check_image(im); }
+
+// The CUDA array behind a surface image: a 2D array (not layered, not 3D) whose element is the format's size and whose extent holds
+// width x height.  An unknown handle: FSR1_ERR_INVALID_ARGUMENT (the failed query's error is cleared: nothing has launched).
+int surface_fits(const fsr1_image* im) {
+  cudaResourceDesc rd;
+  cudaChannelFormatDesc cd;
+  cudaExtent ext;
+  unsigned int aflags = 0;
+  if (cudaGetSurfaceObjectResourceDesc(&rd, (cudaSurfaceObject_t)(uintptr_t)im->data) != cudaSuccess) {
+    cudaGetLastError();
+    return FSR1_ERR_INVALID_ARGUMENT;
+  }
+  if (rd.resType != cudaResourceTypeArray) return FSR1_ERR_UNSUPPORTED;
+  if (cudaArrayGetInfo(&cd, &ext, &aflags, rd.res.array.array) != cudaSuccess) {
+    cudaGetLastError();
+    return FSR1_ERR_INVALID_ARGUMENT;
+  }
+  if (ext.depth != 0 || (aflags & cudaArrayLayered)) return FSR1_ERR_UNSUPPORTED;
+  if ((cd.x + cd.y + cd.z + cd.w) != 8 * bytes_per_pixel(im->format)) return FSR1_ERR_UNSUPPORTED;
+  if (ext.width < im->width || ext.height < im->height) return FSR1_ERR_INVALID_ARGUMENT;
+  return FSR1_OK;
+}
+
+// Every refusal of the surface flags of a call that may take both (fsr1_upscale, fsr1_upscale_post), before anything launches, so that
+// the two-kernel path never runs EASU and then refuses RCAS's store: the flag and format rules first, then the arrays.  unorm_out: the
+// output may also be RGBA8 / RGB10A2 (fsr1_upscale_post's TEPD; its format rules are post_params').  The layouts were checked already.
+int surface_rules(const fsr1_image* in, const fsr1_image* out, const uint32_t* easu_con, uint32_t flags, bool unorm_out) {
+  if (flags & kSurfRefused) return FSR1_ERR_UNSUPPORTED;
+  if (in->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;  // the surface twins are those of the RGBA16F kernels
+  if (flags & FSR1_FLAG_IN_SURFACE) {
+    if (!is_upscale(word_as_float(easu_con[0]), word_as_float(easu_con[1]))) return FSR1_ERR_UNSUPPORTED;  // no direct kernel reads one
+  }
+  if (flags & FSR1_FLAG_OUT_SURFACE) {
+    if (flags & FSR1_FLAG_NO_RCAS) return FSR1_ERR_UNSUPPORTED;  // EASU stores to linear images only
+    const bool ok = out->format == FSR1_FORMAT_RGBA16F ||
+                    (unorm_out && (out->format == FSR1_FORMAT_RGBA8_UNORM || out->format == FSR1_FORMAT_RGB10A2_UNORM));
+    if (!ok) return FSR1_ERR_UNSUPPORTED;
+  }
+  int rc;
+  if ((flags & FSR1_FLAG_IN_SURFACE) && (rc = surface_fits(in)) != FSR1_OK) return rc;
+  if ((flags & FSR1_FLAG_OUT_SURFACE) && (rc = surface_fits(out)) != FSR1_OK) return rc;
+  return FSR1_OK;
+}
 
 bool window_holds(const fsr1_image* im, int first, int last) {  // logical rows [first,last]
   return first >= (int)im->row0 && last < (int)(im->row0 + im->rows);
@@ -125,7 +182,7 @@ RcasParams rcas_params(const fsr1_image* in, const fsr1_image* out, const uint32
 int srtm_input_check(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], uint32_t flags) {
   if (in->format != FSR1_FORMAT_RGBA16F && in->format != FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
   if (flags & (FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE)) return FSR1_ERR_UNSUPPORTED;
-  if (((uintptr_t)in->data & 15) || (in->pitch_bytes & 15)) return FSR1_ERR_UNSUPPORTED;  // TMA
+  if (!(flags & FSR1_FLAG_IN_SURFACE) && (((uintptr_t)in->data & 15) || (in->pitch_bytes & 15))) return FSR1_ERR_UNSUPPORTED;  // TMA
   if (out && (((uintptr_t)out->data & 15) || (out->pitch_bytes & 15))) return FSR1_ERR_UNSUPPORTED;  // 16-byte pixel-pair stores
   if (!is_upscale(word_as_float(con[0]), word_as_float(con[1]))) return FSR1_ERR_UNSUPPORTED;
   return FSR1_OK;
@@ -181,10 +238,11 @@ cudaError_t launch_fused(const fsr1_image* in, const fsr1_image* out, const uint
   EasuParams p = easu_params(in, out, easu_con, y0, y1);
   if (sync) p.sync = *sync;
   const bool srtm_in = (flags & FSR1_FLAG_SRTM_INPUT) != 0, r11 = in->format == FSR1_FORMAT_R11G11B10_FLOAT;
+  const bool surf_in = (flags & FSR1_FLAG_IN_SURFACE) != 0, surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const char* name = "";
-  const cudaError_t e = q ? launch_fused_h_post(p, rcas_con[1], *q, (int)out->format, s, &name, srtm_in, r11)
-                          : launch_fused_h(p, rcas_con[1], 0, s, &name, srtm_in, r11);
+  const cudaError_t e = q ? launch_fused_h_post(p, rcas_con[1], *q, (int)out->format, s, &name, srtm_in, r11, surf_in, surf_out)
+                          : launch_fused_h(p, rcas_con[1], 0, s, &name, srtm_in, r11, surf_in, surf_out);
   if (e != cudaSuccess) return e;
   launched(name);
   if (sync) *sync_taken = true;
@@ -243,8 +301,12 @@ int easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], ui
          const HaloSync* sync, bool* sync_taken) {
   NvtxRange range("EASU");
   int rc;
-  if ((rc = check_image(in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
+  const bool surf_in = (flags & FSR1_FLAG_IN_SURFACE) != 0;
+  if ((rc = check_io(in, surf_in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
   if (!con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
+  if (flags & FSR1_FLAG_OUT_SURFACE) return FSR1_ERR_UNSUPPORTED;  // EASU stores to linear images only
+  if (surf_in && (flags & kSurfRefused)) return FSR1_ERR_UNSUPPORTED;
+  if (surf_in && (in->format != FSR1_FORMAT_RGBA16F || !is_upscale(word_as_float(con[0]), word_as_float(con[1])))) return FSR1_ERR_UNSUPPORTED;
   if (out->format != easu_out_format(in->format)) return FSR1_ERR_UNSUPPORTED;
   const bool r11 = in->format == FSR1_FORMAT_R11G11B10_FLOAT;
   if (r11 && (flags & kR11Refused)) return FSR1_ERR_UNSUPPORTED;
@@ -256,6 +318,7 @@ int easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], ui
   if (!window_holds(in, (int)r0, (int)r1)) return FSR1_ERR_WINDOW;
   const bool srtm_in = (flags & FSR1_FLAG_SRTM_INPUT) != 0;
   if (srtm_in && (rc = srtm_input_check(in, out, con, flags)) != FSR1_OK) return rc;
+  if (surf_in && (rc = surface_fits(in)) != FSR1_OK) return rc;
 
   EasuParams p = easu_params(in, out, con, y0, y1);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -271,11 +334,11 @@ int easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], ui
     if (flags & FSR1_FLAG_PRECISE) e = launch_easu_h_precise(p, s, &name);
     if (e == cudaErrorNotSupported) {
       if (sync) p.sync = *sync;  // sharded frame: the neighbour hand-shake rides inside the kernel
-      e = launch_easu_h_tiled(p, s, &name, srtm_in, r11);
+      e = launch_easu_h_tiled(p, s, &name, srtm_in, r11, surf_in);
       if (e == cudaSuccess && sync) *sync_taken = true;
       p.sync = HaloSync{};
     }
-    if (e == cudaErrorNotSupported && srtm_in) return FSR1_ERR_UNSUPPORTED;  // nothing launched; no other kernel applies the flag
+    if (e == cudaErrorNotSupported && (srtm_in || surf_in)) return FSR1_ERR_UNSUPPORTED;  // nothing launched; no other kernel applies the flag
   } else if (in->format == FSR1_FORMAT_RGBA32F && !exact && !(flags & FSR1_FLAG_FORCE_DIRECT)) {
     e = launch_easu_f32_tiled(p, s, &name);
   } else if ((in->format == FSR1_FORMAT_RGBA8_UNORM || in->format == FSR1_FORMAT_RGB10A2_UNORM) && !exact &&
@@ -300,12 +363,18 @@ int upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, 
       return FSR1_ERR_UNSUPPORTED;
     if (flags & kR11Refused) return FSR1_ERR_UNSUPPORTED;
   }
+  const bool surf_in = (flags & FSR1_FLAG_IN_SURFACE) != 0, surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
+  int rc;
+  if (surf_in || surf_out) {  // every refusal of the surfaces before anything launches
+    if ((rc = check_io(in, surf_in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
+    if (!easu_con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
+    if ((rc = surface_rules(in, out, easu_con, flags, false)) != FSR1_OK) return rc;
+  }
   if (flags & FSR1_FLAG_NO_RCAS) return easu(in, out, easu_con, y0, y1, flags, stream, sync, sync_taken);
   const Rows e = easu_rows(y0, y1, out->height);
   if ((flags & FSR1_FLAG_FUSED) && in && easu_con && rcas_con && (in->format == FSR1_FORMAT_RGBA16F || r11) &&
       out->format == FSR1_FORMAT_RGBA16F && !(flags & kNotFused)) {
-    int rc;
-    if ((rc = check_image(in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
+    if ((rc = check_io(in, surf_in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
     if (flags & ~kAllFlags) return FSR1_ERR_INVALID_ARGUMENT;
     if (y0 >= y1 || y1 > out->height) return FSR1_ERR_INVALID_ARGUMENT;
     if (!window_holds(out, (int)y0, (int)y1 - 1)) return FSR1_ERR_WINDOW;
@@ -319,9 +388,11 @@ int upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, 
   }
   flags &= ~(uint32_t)FSR1_FLAG_FUSED;
   if (!tmp) return FSR1_ERR_INVALID_ARGUMENT;
-  int rc = easu(in, tmp, easu_con, e.a, e.b, flags & ~(uint32_t)FSR1_FLAG_OUTPUT_SQUARE, stream, sync, sync_taken);  // last pass only
+  if (surf_out && (((uintptr_t)tmp->data & 15) || (tmp->pitch_bytes & 15))) return FSR1_ERR_UNSUPPORTED;  // the packed RCAS kernel's loads
+  // the output square and OUT_SURFACE belong to the last pass, SRTM_INPUT and IN_SURFACE to EASU's load stage
+  rc = easu(in, tmp, easu_con, e.a, e.b, flags & ~(uint32_t)(FSR1_FLAG_OUTPUT_SQUARE | FSR1_FLAG_OUT_SURFACE), stream, sync, sync_taken);
   if (rc != FSR1_OK) return rc;
-  return fsr1_rcas(tmp, out, rcas_con, y0, y1, flags & ~(uint32_t)FSR1_FLAG_SRTM_INPUT, stream);  // EASU's load stage only
+  return fsr1_rcas(tmp, out, rcas_con, y0, y1, flags & ~(uint32_t)(FSR1_FLAG_SRTM_INPUT | FSR1_FLAG_IN_SURFACE), stream);
 }
 
 int upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, const uint32_t easu_con[16],
@@ -330,7 +401,8 @@ int upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
   if (!post || post->ops == 0) return upscale(in, tmp, out, easu_con, rcas_con, y0, y1, flags, stream, sync, sync_taken);
   NvtxRange range("FSR1 upscale post");
   int rc;
-  if ((rc = check_image(in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
+  const bool surf_in = (flags & FSR1_FLAG_IN_SURFACE) != 0, surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
+  if ((rc = check_io(in, surf_in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
   if (!easu_con || !rcas_con) return FSR1_ERR_INVALID_ARGUMENT;
   PostParams q;
   if ((rc = post_params(post, in->format, out->format, flags, q)) != FSR1_OK) return rc;
@@ -343,15 +415,16 @@ int upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
   fsr1_easu_input_rows(easu_con, in->height, e.a, e.b, &r0, &r1);
   if (!window_holds(in, (int)r0, (int)r1)) return FSR1_ERR_WINDOW;
   const int out_align = out->format == FSR1_FORMAT_RGBA16F ? 16 : 8;
-  if (((uintptr_t)out->data & (out_align - 1)) || (out->pitch_bytes & (out_align - 1))) return FSR1_ERR_UNSUPPORTED;
+  if (!surf_out && (((uintptr_t)out->data & (out_align - 1)) || (out->pitch_bytes & (out_align - 1)))) return FSR1_ERR_UNSUPPORTED;
   if (tmp) {  // the intermediate of the two-kernel path (unused by the fused kernel)
     if ((rc = check_image(tmp)) != FSR1_OK) return rc;
     if (tmp->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
     if (tmp->width != out->width || tmp->height != out->height) return FSR1_ERR_INVALID_ARGUMENT;
     if (!window_holds(tmp, (int)e.a, (int)e.b - 1)) return FSR1_ERR_WINDOW;
     if (((uintptr_t)tmp->data & 15) || (tmp->pitch_bytes & 15)) return FSR1_ERR_UNSUPPORTED;
-    if (overlaps(tmp, out)) return FSR1_ERR_INVALID_ARGUMENT;
+    if (!surf_out && overlaps(tmp, out)) return FSR1_ERR_INVALID_ARGUMENT;
   }
+  if ((surf_in || surf_out) && (rc = surface_rules(in, out, easu_con, flags, true)) != FSR1_OK) return rc;
   if ((flags & FSR1_FLAG_FUSED) && !(flags & kNotFused)) {
     const cudaError_t err = launch_fused(in, out, easu_con, rcas_con, &q, y0, y1, flags, stream, sync, sync_taken);
     if (err == cudaSuccess) return FSR1_OK;
@@ -359,12 +432,13 @@ int upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
   }
   // EASU into tmp (as fsr1_upscale does), then RCAS with the epilogue in its store
   if (!tmp) return FSR1_ERR_INVALID_ARGUMENT;
-  rc = easu(in, tmp, easu_con, e.a, e.b, flags & ~(uint32_t)(FSR1_FLAG_FUSED | FSR1_FLAG_OUTPUT_SQUARE), stream, sync, sync_taken);
+  rc = easu(in, tmp, easu_con, e.a, e.b, flags & ~(uint32_t)(FSR1_FLAG_FUSED | FSR1_FLAG_OUTPUT_SQUARE | FSR1_FLAG_OUT_SURFACE), stream, sync,
+            sync_taken);
   if (rc != FSR1_OK) return rc;
   RcasParams p = rcas_params(tmp, out, rcas_con, y0, y1, flags);
   p.options |= (flags & FSR1_FLAG_OUTPUT_SQUARE) ? 4 : 0;
   const char* name = "";
-  const cudaError_t err = launch_rcas_h_post(p, q, (int)out->format, static_cast<cudaStream_t>(stream), &name);
+  const cudaError_t err = launch_rcas_h_post(p, q, (int)out->format, static_cast<cudaStream_t>(stream), &name, surf_out);
   if (err != cudaSuccess) return err == cudaErrorNotSupported ? FSR1_ERR_UNSUPPORTED : cuda_fail(err);
   launched(name);
   return FSR1_OK;
@@ -429,9 +503,12 @@ int fsr1_rcas(const fsr1_image* in, const fsr1_image* out, const uint32_t con[4]
               uint32_t flags, void* stream) {
   NvtxRange range("RCAS");
   int rc;
-  if ((rc = check_image(in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
+  const bool surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
+  if ((rc = check_image(in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
   if (!con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
   if (flags & FSR1_FLAG_SRTM_INPUT) return FSR1_ERR_INVALID_ARGUMENT;  // RCAS has no input stage
+  if (flags & FSR1_FLAG_IN_SURFACE) return FSR1_ERR_UNSUPPORTED;      // RCAS reads the linear intermediate
+  if (surf_out && ((flags & kSurfRefused) || out->format != FSR1_FORMAT_RGBA16F)) return FSR1_ERR_UNSUPPORTED;
   if (in->format != out->format || in->format == FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
   if (in->width != out->width || in->height != out->height) return FSR1_ERR_INVALID_ARGUMENT;
   if (y1 == 0) y1 = out->height;
@@ -439,7 +516,8 @@ int fsr1_rcas(const fsr1_image* in, const fsr1_image* out, const uint32_t con[4]
   if (!window_holds(out, (int)y0, (int)y1 - 1)) return FSR1_ERR_WINDOW;
   const Rows need = easu_rows(y0, y1, out->height);
   if (!window_holds(in, (int)need.a, (int)need.b - 1)) return FSR1_ERR_WINDOW;
-  if (overlaps(in, out)) return FSR1_ERR_INVALID_ARGUMENT;
+  if (!surf_out && overlaps(in, out)) return FSR1_ERR_INVALID_ARGUMENT;
+  if (surf_out && (rc = surface_fits(out)) != FSR1_OK) return rc;
 
   RcasParams p = rcas_params(in, out, con, y0, y1, flags);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -456,8 +534,9 @@ int fsr1_rcas(const fsr1_image* in, const fsr1_image* out, const uint32_t con[4]
     e = launch_rcas_href(p, s, &name);
   } else if (in->format == FSR1_FORMAT_RGBA16F && !exact && !(flags & FSR1_FLAG_FORCE_DIRECT)) {
     p.options |= fused_square;  // the reference's options are template bits of the packed kernels: no slower fallback
-    e = launch_rcas_h_packed(p, s, &name);
+    e = launch_rcas_h_packed(p, s, &name, surf_out);
     squared = e == cudaSuccess;
+    if (e == cudaErrorNotSupported && surf_out) return FSR1_ERR_UNSUPPORTED;  // nothing launched; no other kernel writes a surface
   } else if (in->format == FSR1_FORMAT_RGBA32F && !exact && !(flags & FSR1_FLAG_FORCE_DIRECT)) {
     p.options |= fused_square;
     e = launch_rcas_f32_packed(p, s, &name);
@@ -600,6 +679,7 @@ int fsr1_context_upscale(fsr1_context* c, const void* in_dev, uint64_t in_pitch,
 int fsr1_context_upscale_host(fsr1_context* c, const void* in_host, uint64_t in_pitch, void* out_host,
                               uint64_t out_pitch, float sharpness, uint32_t flags, void* stream) {
   if (!c || !in_host || !out_host) return FSR1_ERR_INVALID_ARGUMENT;
+  if (flags & kSurfFlags) return FSR1_ERR_UNSUPPORTED;  // its frames are host memory, staged through the context's linear buffers
   const uint64_t bpp = (uint64_t)bytes_per_pixel(c->format), obpp = (uint64_t)bytes_per_pixel(easu_out_format(c->format));
   if (in_pitch < c->in_w * bpp || out_pitch < c->out_w * obpp) return FSR1_ERR_INVALID_ARGUMENT;
   cudaError_t e;

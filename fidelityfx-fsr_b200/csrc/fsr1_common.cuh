@@ -264,6 +264,26 @@ __device__ __forceinline__ void halo_sync_end(const HaloSync& hs) {
 
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(max(v, lo), hi); }
 
+// ---- surface access (FSR1_FLAG_IN_SURFACE / FSR1_FLAG_OUT_SURFACE) ---------------------------------------------------------
+// A surface image's ImgView holds the cudaSurfaceObject_t in `base` (pitch 0, row0 0, rows = h).  x is a pixel index here and a byte
+// offset in the instruction.  Zero mode: an access outside the array reads 0 and a store there is dropped; callers clamp to the
+// LOGICAL image themselves and never rely on it (trap mode would turn a coordinate bug into a fault).  tests/emu supplies these
+// wrappers under FSR1_CPU_EMU (fsr1_emu_surf.h), as it does the PTX wrappers of fsr1_easu_common.cuh.
+#ifdef FSR1_CPU_EMU
+}  // namespace fsr1
+#include "fsr1_emu_surf.h"
+namespace fsr1 {
+#else
+__device__ __forceinline__ unsigned long long surf_of(const ImgView& im) { return (unsigned long long)im.base; }
+__device__ __forceinline__ uint2 surf_load8(unsigned long long s, int x, int y) {
+  return surf2Dread<uint2>(s, x * 8, y, cudaBoundaryModeZero);
+}
+__device__ __forceinline__ void surf_store8(unsigned long long s, int x, int y, uint2 v) { surf2Dwrite(v, s, x * 8, y, cudaBoundaryModeZero); }
+__device__ __forceinline__ void surf_store4(unsigned long long s, int x, int y, uint32_t v) {
+  surf2Dwrite(v, s, x * 4, y, cudaBoundaryModeZero);
+}
+#endif
+
 // ---- host helpers of the dispatch layer (fsr1_capi.cu, fsr1_shard.cu) -----------------------------------------------------
 inline int bytes_per_pixel(uint32_t fmt) {  // 0: not a format include/fsr1_b200.h defines
   switch (fmt) {
@@ -305,14 +325,17 @@ cudaError_t launch_rcas_direct(const RcasParams& p, int format, bool exact, cuda
 // meet their alignment needs (the caller then falls back to the direct kernels).  srtm_in: FSR1_FLAG_SRTM_INPUT (the caller
 // must not fall back then: no other kernel applies it).
 // r11: the input is R11G11B10_FLOAT (the output RGBA16F); no fall-back either (launch_easu_direct decodes the format itself).
-cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in = false, bool r11 = false);
-cudaError_t launch_rcas_h_packed(const RcasParams& p, cudaStream_t s, const char** name);
+// surf_in (FSR1_FLAG_IN_SURFACE): p.in.base is a surface object on an RGBA16F array; surf_out (FSR1_FLAG_OUT_SURFACE): p.out.base is one.
+// No fall-back for either: no other kernel reads or writes a surface.
+cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in = false, bool r11 = false,
+                                bool surf_in = false);
+cudaError_t launch_rcas_h_packed(const RcasParams& p, cudaStream_t s, const char** name, bool surf_out = false);
 // UNORM images through the TMA-tiled 2x EASU / packed RCAS kernels: cudaErrorNotSupported when not applicable
 cudaError_t launch_easu_u_tiled(const EasuParams& p, int format, cudaStream_t s, const char** name);
 cudaError_t launch_rcas_u_packed(const RcasParams& p, int format, cudaStream_t s, const char** name);
 // EASU -> RCAS in one kernel (RGBA16F, exactly 2x, out-of-image taps read 0): e.in = input, e.out = final output, rows [e.y0, e.y1)
 cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in = false,
-                           bool r11 = false);
+                           bool r11 = false, bool surf_in = false, bool surf_out = false);
 cudaError_t launch_easu_f32_tiled(const EasuParams& p, cudaStream_t s, const char** name);  // RGBA32F, exactly 2x
 cudaError_t launch_easu_h_precise(const EasuParams& p, cudaStream_t s, const char** name);  // RGBA16F io, fp32 math, 2x
 cudaError_t launch_rcas_f32_packed(const RcasParams& p, cudaStream_t s, const char** name);

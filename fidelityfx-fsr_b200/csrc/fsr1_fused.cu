@@ -134,7 +134,8 @@ template <int CY> struct FusedIter {
 // (see the caller): no pixel masked, every store a full pair, no row skipped but the first two of a run's first step — a
 // predicate-free copy of the body, as easu_h_quad2x_kernel takes for interior tiles.
 // SO: void = RCAS's own RGBA16F store; otherwise the display epilogue of fsr1_upscale_post (post_pair, fsr1_post.cuh) with its store.
-template <bool kIn, int NW, typename SO>
+// kSurfOut (FSR1_FLAG_OUT_SURFACE): p.out.base is a surface object; each output pixel is one surface store of its element at (x, row).
+template <bool kIn, int NW, typename SO, bool kSurfOut = false>
 __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams& p, const FusedStep& cur, const uint2* tile, int dx,
                                            int k0, __half2 sharp, int lane, int warp, const PostParams* q) {
   constexpr int CY = FusedCfg<NW>::kCY;
@@ -163,8 +164,9 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
   const bool writer = lane >= 1 && (kIn || ox < p.out.w);
   // kIn: only the first two rows of a run's first step (warp 0) lie above ya; they are computed like the others, not stored
   const bool wtop = writer && (!kIn || o_first >= cur.ya);
-  if constexpr (kPost) {
-    // the epilogue needs registers: a rolling window of three mid rows instead of all kR + 2 up front (no spills at 6 CTAs per SM)
+  if constexpr (kPost || kSurfOut) {
+    // the epilogue needs registers: a rolling window of three mid rows instead of all kR + 2 up front (no spills at 6 CTAs per SM);
+    // the surface stores take the same window (surf_per_sm)
     auto mid_row = [&](int i, Row3& e, Row3& d, Row3& f) {
       const uint4 a = sm.mid[i][lm], c = sm.mid[i][lane];
       e.r = uh2(__byte_perm(a.x, c.x, 0x5432));
@@ -178,7 +180,7 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
     mid_row(i0 + 1, eb, db, fb);
     unsigned char* dst = p.out.base + (long long)(o_first - p.out.row0) * p.out.pitch + (long long)ox * PostStore<SO>::kBytes;
     PostCursor pc;
-    pc.init(*q, ox, o_first);
+    if constexpr (kPost) pc.init(*q, ox, o_first);
 #pragma unroll
     for (int r = 0; r < kR; r++) {
       const int o = o_first + r;
@@ -186,9 +188,18 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
       if (kIn || (o >= cur.ya && o < cur.yb && o < 2 * cur.m0 + 2 * n)) {  // warp-uniform
         __half2 oR, oG, oB;
         rcas_pair<0>(ea, db, eb, fb, ec, sharp, oR, oG, oB);
-        if (r >= 2 ? writer : wtop) post_pair<SO>(*q, pc, dst + (long long)r * p.out.pitch, ox, o, oR, oG, oB, 0x3c003c00u, kIn || ox + 1 < p.out.w);
+        if (r >= 2 ? writer : wtop) {
+          if constexpr (kPost) {
+            post_pair<SO, kSurfOut>(*q, pc, kSurfOut ? p.out.base : dst + (long long)r * p.out.pitch, ox, o, oR, oG, oB, 0x3c003c00u,
+                                    kIn || ox + 1 < p.out.w);
+          } else {
+            const uint4 w = pack_pair_half(oR, oG, oB, 0x3c003c00u);
+            surf_store8(surf_of(p.out), ox, o, make_uint2(w.x, w.y));
+            if (kIn || ox + 1 < p.out.w) surf_store8(surf_of(p.out), ox + 1, o, make_uint2(w.z, w.w));
+          }
+        }
       }
-      pc.next_row(*q);
+      if constexpr (kPost) pc.next_row(*q);
       ea = eb; eb = ec; db = dc; fb = fc;
     }
   } else {
@@ -222,7 +233,10 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
   }
 }
 
-template <int NW, typename SO, bool kSrtmIn, bool kR11 = false>
+// kSurfIn (FSR1_FLAG_IN_SURFACE): p.in.base is a surface object on an RGBA16F array and `tmap` is unused.  Phase 1 reads the step's
+// kFBW (n + 3) texels with surface loads at coordinates clamped to the logical image (the texels TMA + clamp_fixup would leave in the
+// tile), into one tile buffer: no TMA, no mbarrier, no prefetch.  The previous step's closing barrier frees the buffer.
+template <int NW, typename SO, bool kSrtmIn, bool kR11 = false, bool kSurfIn = false, bool kSurfOut = false>
 __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMap& tmap, const PostParams* q) {
   using C = FusedCfg<NW>;
   constexpr int NT = NW * 32, CY = C::kCY;
@@ -235,12 +249,14 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
     stage = &r11_stage.w[0][0];
   }
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) {
-    mbar_init(&sm.bar[0], 1);
-    mbar_init(&sm.bar[1], 1);
-    mbar_fence_init();
+  if (!kSurfIn) {
+    if (tid == 0) {
+      mbar_init(&sm.bar[0], 1);
+      mbar_init(&sm.bar[1], 1);
+      mbar_fence_init();
+    }
+    __syncthreads();
   }
-  __syncthreads();
   halo_sync_begin(p.sync);
   FusedIter<CY> iter;
   iter.init(p, blockIdx.x, gridDim.x);
@@ -248,7 +264,7 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
   bool has = iter.next(cur);
   auto box_x = [](const FusedStep& s) { return (kStripCells * s.tx - 2) & ~1; };  // even texel at or before the first tap column
   auto tma_x = [&](const FusedStep& s) { return kR11 ? box_x(s) & ~3 : box_x(s); };
-  if (tid == 0 && has) {
+  if (!kSurfIn && tid == 0 && has) {
     mbar_expect_tx(&sm.bar[0], kBoxBytes);
     tma_load_2d(kR11 ? (void*)stage : (void*)sm.tile[0], &tmap, tma_x(cur), cur.m0 - 1 - p.in.row0, &sm.bar[0]);
   }
@@ -256,25 +272,36 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
   for (int it = 0; has; it++) {
     const int b = it & 1;
     const bool hasn = iter.next(nxt);
-    if (tid == 0 && hasn) {  // prefetch the next step's box into the other buffer (its readers passed the closing barrier)
+    if (!kSurfIn && tid == 0 && hasn) {  // prefetch the next step's box into the other buffer (its readers passed the closing barrier)
       fence_proxy_async();
       mbar_expect_tx(&sm.bar[b ^ 1], kBoxBytes);
       tma_load_2d(kR11 ? (void*)(stage + (b ^ 1) * kStage) : (void*)sm.tile[b ^ 1], &tmap, tma_x(nxt), nxt.m0 - 1 - p.in.row0,
                   &sm.bar[b ^ 1]);
     }
-    uint2* tile = sm.tile[kR11 ? 0 : b];  // kR11: phase 1 writes the half tile after the previous step's closing barrier
+    uint2* tile = sm.tile[kR11 || kSurfIn ? 0 : b];  // kR11, kSurfIn: phase 1 writes the half tile after the previous step's closing barrier
     const int k0 = kStripCells * cur.tx - 1;       // first cell of the strip (lane 0)
     const int gxe = box_x(cur), dx = (k0 - 1) - gxe;  // box origin; offset of tap column 0 of lane 0 inside it (0 or 1)
     const int gy0 = cur.m0 - 1, n = cur.n;
-    mbar_wait(&sm.bar[b], (it >> 1) & 1);
-    if (gxe < 0 || gy0 < 0 || gxe + kFBW > p.in.w || gy0 + C::kBH > p.in.h) {
-      if constexpr (kR11) clamp_fixup(stage + b * kStage + (gxe & 3), kRBW, kFBW, C::kBH, gxe, gy0, p.in.w, p.in.h, lane, warp, NW);
-      else clamp_fixup(tile, kFBW, kFBW, C::kBH, gxe, gy0, p.in.w, p.in.h, lane, warp, NW);
-      fence_proxy_async();
-      __syncthreads();
+    if (!kSurfIn) {
+      mbar_wait(&sm.bar[b], (it >> 1) & 1);
+      if (gxe < 0 || gy0 < 0 || gxe + kFBW > p.in.w || gy0 + C::kBH > p.in.h) {
+        if constexpr (kR11) clamp_fixup(stage + b * kStage + (gxe & 3), kRBW, kFBW, C::kBH, gxe, gy0, p.in.w, p.in.h, lane, warp, NW);
+        else clamp_fixup(tile, kFBW, kFBW, C::kBH, gxe, gy0, p.in.w, p.in.h, lane, warp, NW);
+        fence_proxy_async();
+        __syncthreads();
+      }
     }
     // phases 1 and 2 on the rows this step needs (n + 3 texel rows, n + 1 rows of terms)
-    if constexpr (kR11) {
+    if constexpr (kSurfIn) {
+      const unsigned long long src = surf_of(p.in);
+      for (int i = tid; i < kFBW * (n + 3); i += NT) {
+        const int j = i / kFBW, c = i - j * kFBW;
+        uint2 t = surf_load8(src, clampi(gxe + c, 0, p.in.w - 1), clampi(gy0 + j, 0, p.in.h - 1));
+        if (kSrtmIn) t = srtm_texel(t);
+        tile[i] = t;
+        sm.L[i] = texel_luma(t);
+      }
+    } else if constexpr (kR11) {
       r11_phase1_staged<kSrtmIn, NT>(stage + b * kStage, tile, sm.L, kFBW * (n + 3), kFBW, kRBW, gxe & 3, tid);
     } else {
       for (int i = tid; i < kFBW * (n + 3); i += NT) {
@@ -295,8 +322,8 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
     // above ya (fused_step skips them)
     const bool inside = k0 >= 0 && 2 * (k0 + 31) + 2 < p.out.w && cur.m0 >= 0 && 2 * (cur.m0 + CY) < p.out.h && n == CY &&
                         2 * cur.m0 + 2 >= cur.ya && 2 * (cur.m0 + CY) <= cur.yb;
-    if (inside) fused_step<true, NW, SO>(sm, p, cur, tile, dx, k0, sharp, lane, warp, q);
-    else fused_step<false, NW, SO>(sm, p, cur, tile, dx, k0, sharp, lane, warp, q);
+    if (inside) fused_step<true, NW, SO, kSurfOut>(sm, p, cur, tile, dx, k0, sharp, lane, warp, q);
+    else fused_step<false, NW, SO, kSurfOut>(sm, p, cur, tile, dx, k0, sharp, lane, warp, q);
     __syncthreads();
     if (n == CY && tid < 64) {  // the run may continue: its last two mid rows become rows 0, 1 of the next step
       const int rr = tid >> 5;
@@ -335,24 +362,40 @@ fused_r11_quad2x_post_kernel(const FusedParams p, const __grid_constant__ CUtens
   fused_body<NW, SO, kSrtmIn, true>(p, tmap, &q);
 }
 
+// FSR1_FLAG_IN_SURFACE / OUT_SURFACE: the same two kernels reading the input and / or writing the output through surface objects
+// (RGBA16F input; `tmap` is unused with kSurfIn)
+template <int NW, int MINB, bool kSrtmIn, bool kSurfIn, bool kSurfOut>
+__global__ void __launch_bounds__(NW * 32, MINB)
+fused_h_quad2x_surf_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap) {
+  fused_body<NW, void, kSrtmIn, false, kSurfIn, kSurfOut>(p, tmap, nullptr);
+}
+template <int NW, int MINB, typename SO, bool kSrtmIn, bool kSurfIn, bool kSurfOut>
+__global__ void __launch_bounds__(NW * 32, MINB)
+fused_h_quad2x_post_surf_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap, const __grid_constant__ PostParams q) {
+  fused_body<NW, SO, kSrtmIn, false, kSurfIn, kSurfOut>(p, tmap, &q);
+}
+
 #ifndef FSR1_CPU_EMU
 // tensor map, parameters and grid of a fused launch; cudaErrorNotSupported when the frame is not one the kernel takes.
-// out_align: the alignment the output store needs (16 for RGBA16F pairs, 8 for UNORM pairs).
+// out_align: the alignment the output store needs (16 for RGBA16F pairs, 8 for UNORM pairs).  surf_in / surf_out: that side is a
+// surface object (no alignment rule; no tensor map for a surface input: `tmap` is zeroed).
 static cudaError_t fused_setup(const EasuParams& e, uint32_t sharp_h2, int out_align, bool r11, CUtensorMap& tmap, FusedParams& p,
-                               int& per_sm, long long& grid) {
+                               int& per_sm, long long& grid, bool surf_in = false, bool surf_out = false) {
   if (!is_2x(e.c0x, e.c0y, e.c0z, e.c0w)) return cudaErrorNotSupported;
-  if ((reinterpret_cast<uintptr_t>(e.in.base) & 15) || (e.in.pitch & 15) || (reinterpret_cast<uintptr_t>(e.out.base) & (out_align - 1)) ||
-      (e.out.pitch & (out_align - 1)))
+  if ((!surf_in && ((reinterpret_cast<uintptr_t>(e.in.base) & 15) || (e.in.pitch & 15))) ||
+      (!surf_out && ((reinterpret_cast<uintptr_t>(e.out.base) & (out_align - 1)) || (e.out.pitch & (out_align - 1)))))
     return cudaErrorNotSupported;
   constexpr int NW = 4;
   using C = FusedCfg<NW>;
   EncodeTiledFn encode = get_encode_fn();
-  if (!encode) return cudaErrorNotSupported;
+  if (surf_in) memset(&tmap, 0, sizeof tmap);
+  else if (!encode) return cudaErrorNotSupported;
   const cuuint64_t dims[2] = {(cuuint64_t)e.in.w, (cuuint64_t)e.in.rows};
   const cuuint64_t strides[1] = {(cuuint64_t)e.in.pitch};
   const cuuint32_t box[2] = {(cuuint32_t)(r11 ? kRBW : kFBW), (cuuint32_t)C::kBH};
   const cuuint32_t estr[2] = {1, 1};
-  if (encode(&tmap, r11 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, e.in.base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  if (!surf_in &&
+      encode(&tmap, r11 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, e.in.base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
     return cudaErrorNotSupported;
   p.in = e.in; p.out = e.out; p.y0 = e.y0; p.y1 = e.y1; p.sharp_h2 = sharp_h2; p.sync = e.sync;
@@ -368,14 +411,73 @@ static cudaError_t fused_setup(const EasuParams& e, uint32_t sharp_h2, int out_a
   return cudaSuccess;
 }
 
-cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in, bool r11) {
+// The display epilogue needs more registers than the 72 of 7 CTAs per SM (-Xptxas -v: DESIGN.md §4): 6 per SM.
+constexpr int kPostPerSm = 6;
+
+// FSR1_FLAG_IN_SURFACE / OUT_SURFACE: the surface twin of the plain (SO = void) or post kernel for the flag combination.  The plain twin
+// that takes its input by TMA and stores through a surface spills 4-8 B at the 72 registers of 7 CTAs per SM (-Xptxas -v, rolled or
+// unrolled row loop), so it runs at 6 per SM; the others keep 7.
+constexpr int surf_per_sm(bool surf_in, bool surf_out) { return surf_out && !surf_in ? 6 : 7; }
+template <typename SO, bool kSrtmIn, bool kSurfIn, bool kSurfOut>
+static void surf_kernel(const FusedParams& p, const CUtensorMap& tmap, const PostParams* q, long long grid, cudaStream_t s) {
+  if constexpr (std::is_void<SO>::value)
+    fused_h_quad2x_surf_kernel<4, surf_per_sm(kSurfIn, kSurfOut), kSrtmIn, kSurfIn, kSurfOut><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
+  else fused_h_quad2x_post_surf_kernel<4, kPostPerSm, SO, kSrtmIn, kSurfIn, kSurfOut><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, *q);
+}
+// names[0]: plain; [1..3]: post into RGBA16F, RGBA8, RGB10A2.  Index within a row: the combination (srtm_in, surf_in, surf_out) in the
+// order of the switch below.
+static const char* const kSurfNames[4][6] = {
+    {"fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,surf_in>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,surf_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,srtm_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,srtm_in,surf_in>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,srtm_in,surf_in,surf_out>"},
+    {"fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,surf_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,surf_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba16f,srtm_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,srtm_in,surf_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,srtm_in,surf_in,surf_out>"},
+    {"fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,surf_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,surf_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgba8,srtm_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,srtm_in,surf_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,srtm_in,surf_in,surf_out>"},
+    {"fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,surf_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,surf_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,tma2,strips,post,rgb10a2,srtm_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,srtm_in,surf_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,srtm_in,surf_in,surf_out>"}};
+template <typename SO>
+static cudaError_t launch_surf(const FusedParams& p, const CUtensorMap& tmap, const PostParams* q, long long grid, bool srtm_in, bool surf_in,
+                               bool surf_out, cudaStream_t s, const char** name, int names_row) {
+  int v = 0;
+  switch ((srtm_in ? 4 : 0) | (surf_in ? 2 : 0) | (surf_out ? 1 : 0)) {
+    case 1: surf_kernel<SO, false, false, true>(p, tmap, q, grid, s); v = 0; break;
+    case 2: surf_kernel<SO, false, true, false>(p, tmap, q, grid, s); v = 1; break;
+    case 3: surf_kernel<SO, false, true, true>(p, tmap, q, grid, s); v = 2; break;
+    case 5: surf_kernel<SO, true, false, true>(p, tmap, q, grid, s); v = 3; break;
+    case 6: surf_kernel<SO, true, true, false>(p, tmap, q, grid, s); v = 4; break;
+    case 7: surf_kernel<SO, true, true, true>(p, tmap, q, grid, s); v = 5; break;
+    default: return cudaErrorNotSupported;
+  }
+  *name = kSurfNames[names_row][v];
+  return cudaGetLastError();
+}
+
+cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in, bool r11,
+                           bool surf_in, bool surf_out) {
   if (clamp) return cudaErrorNotSupported;
   CUtensorMap tmap;
   FusedParams p;
-  int per_sm = 7;
+  int per_sm = surf_per_sm(surf_in, surf_out);
   long long grid = 0;
-  const cudaError_t err = fused_setup(e, sharp_h2, 16, r11, tmap, p, per_sm, grid);
+  const cudaError_t err = fused_setup(e, sharp_h2, 16, r11, tmap, p, per_sm, grid, surf_in, surf_out);
   if (err != cudaSuccess) return err;
+  if (surf_in || surf_out) return launch_surf<void>(p, tmap, nullptr, grid, srtm_in, surf_in, surf_out, s, name, 0);  // RGBA16F input
   if (r11 && srtm_in) {
     fused_r11_quad2x_kernel<4, 7, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
     *name = per_sm == 7 ? "fused_easu_rcas_h_quad2x<4w,7/sm,tma2,strips,r11g11b10f_in,srtm_in>"
@@ -392,9 +494,6 @@ cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cu
   }
   return cudaGetLastError();
 }
-
-// The display epilogue needs more registers than the 72 of 7 CTAs per SM (-Xptxas -v: DESIGN.md §4): 6 per SM.
-constexpr int kPostPerSm = 6;
 
 // the post kernel for out_format (1 RGBA16F, 3 RGBA8_UNORM, 4 RGB10A2_UNORM) and input kind; its name through *name
 template <bool kSrtmIn, bool kR11>
@@ -433,14 +532,21 @@ static cudaError_t launch_post_kernel(const FusedParams& p, const CUtensorMap& t
 }
 
 cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const PostParams& q, int out_format, cudaStream_t s,
-                                const char** name, bool srtm_in, bool r11) {
+                                const char** name, bool srtm_in, bool r11, bool surf_in, bool surf_out) {
   if (out_format != 1 && out_format != 3 && out_format != 4) return cudaErrorNotSupported;
   CUtensorMap tmap;
   FusedParams p;
   int per_sm = kPostPerSm;
   long long grid = 0;
-  const cudaError_t err = fused_setup(e, sharp_h2, out_format == 1 ? 16 : 8, r11, tmap, p, per_sm, grid);
+  const cudaError_t err = fused_setup(e, sharp_h2, out_format == 1 ? 16 : 8, r11, tmap, p, per_sm, grid, surf_in, surf_out);
   if (err != cudaSuccess) return err;
+  if (surf_in || surf_out) {  // RGBA16F input
+    switch (out_format) {
+      case 1: return launch_surf<__half>(p, tmap, &q, grid, srtm_in, surf_in, surf_out, s, name, 1);
+      case 3: return launch_surf<Unorm8>(p, tmap, &q, grid, srtm_in, surf_in, surf_out, s, name, 2);
+      default: return launch_surf<Unorm10>(p, tmap, &q, grid, srtm_in, surf_in, surf_out, s, name, 3);
+    }
+  }
   if (r11) return srtm_in ? launch_post_kernel<true, true>(p, tmap, q, out_format, grid, s, name)
                           : launch_post_kernel<false, true>(p, tmap, q, out_format, grid, s, name);
   return srtm_in ? launch_post_kernel<true, false>(p, tmap, q, out_format, grid, s, name)

@@ -169,7 +169,7 @@ __device__ __forceinline__ void post_steps(const PostParams& q, float4& c0, floa
 }
 
 // Output store of the epilogue for the pixel pair (x, x+1): SO = __half (RGBA16F, 16 B), Unorm8 or Unorm10 (8 B).  `both`: x+1 is
-// inside the image.  The encodings are Px<SO>::store's.
+// inside the image.  The encodings are Px<SO>::store's.  store_surf: the same bytes through a surface object, one store per pixel.
 template <typename SO> struct PostStore;
 template <> struct PostStore<void> { static constexpr int kBytes = 8; };  // no epilogue: the RGBA16F store of RCAS itself
 template <> struct PostStore<__half> {
@@ -182,6 +182,14 @@ template <> struct PostStore<__half> {
     if (both) *reinterpret_cast<uint4*>(o) = w;
     else *reinterpret_cast<uint2*>(o) = make_uint2(w.x, w.y);
   }
+  static __device__ __forceinline__ void store_surf(unsigned long long s, int x, int y, float4 c0, float4 c1, bool both) {
+    const __half2 rg0 = __floats2half2_rn(c0.x, c0.y), ba0 = __floats2half2_rn(c0.z, c0.w);
+    surf_store8(s, x, y, make_uint2(*reinterpret_cast<const uint32_t*>(&rg0), *reinterpret_cast<const uint32_t*>(&ba0)));
+    if (both) {
+      const __half2 rg1 = __floats2half2_rn(c1.x, c1.y), ba1 = __floats2half2_rn(c1.z, c1.w);
+      surf_store8(s, x + 1, y, make_uint2(*reinterpret_cast<const uint32_t*>(&rg1), *reinterpret_cast<const uint32_t*>(&ba1)));
+    }
+  }
 };
 template <> struct PostStore<Unorm8> {
   static constexpr int kBytes = 4;
@@ -191,6 +199,10 @@ template <> struct PostStore<Unorm8> {
   static __device__ __forceinline__ void store(unsigned char* o, float4 c0, float4 c1, bool both) {
     if (both) *reinterpret_cast<uint2*>(o) = make_uint2(enc(c0), enc(c1));
     else *reinterpret_cast<uint32_t*>(o) = enc(c0);
+  }
+  static __device__ __forceinline__ void store_surf(unsigned long long s, int x, int y, float4 c0, float4 c1, bool both) {
+    surf_store4(s, x, y, enc(c0));
+    if (both) surf_store4(s, x + 1, y, enc(c1));
   }
 };
 template <> struct PostStore<Unorm10> {
@@ -202,24 +214,32 @@ template <> struct PostStore<Unorm10> {
     if (both) *reinterpret_cast<uint2*>(o) = make_uint2(enc(c0), enc(c1));
     else *reinterpret_cast<uint32_t*>(o) = enc(c0);
   }
+  static __device__ __forceinline__ void store_surf(unsigned long long s, int x, int y, float4 c0, float4 c1, bool both) {
+    surf_store4(s, x, y, enc(c0));
+    if (both) surf_store4(s, x + 1, y, enc(c1));
+  }
 };
 
 // RCAS result of the pair (SoA half2, alpha = (A0, A1) as half2 bits, exactly what the RGBA16F store would write) -> post steps ->
-// the output store.  y: the logical output row; k: the pair's tile positions on that row.
-template <typename SO>
+// the output store.  y: the logical output row; k: the pair's tile positions on that row.  o: the pair's address, or with kSurfOut
+// the output's ImgView::base (the surface object), stored to at (x, y).
+template <typename SO, bool kSurfOut = false>
 __device__ __forceinline__ void post_pair(const PostParams& q, const PostCursor& k, unsigned char* o, int x, int y, __half2 oR, __half2 oG,
                                           __half2 oB, uint32_t alpha, bool both) {
   const float2 r = __half22float2(oR), g = __half22float2(oG), b = __half22float2(oB);
   const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&alpha));
   float4 c0 = make_float4(r.x, g.x, b.x, a.x), c1 = make_float4(r.y, g.y, b.y, a.y);
   post_steps(q, c0, c1, x, y, k);
-  PostStore<SO>::store(o, c0, c1, both);
+  if constexpr (kSurfOut) PostStore<SO>::store_surf((unsigned long long)o, x, y, c0, c1, both);
+  else PostStore<SO>::store(o, c0, c1, both);
 }
 
 // launchers (fsr1_fused.cu, fsr1_rcas_packed.cu); out_format 1 RGBA16F, 3 RGBA8_UNORM, 4 RGB10A2_UNORM.  cudaErrorNotSupported: the
 // frame or layout is not one the kernel takes (nothing launched).
+// surf_in / surf_out: FSR1_FLAG_IN_SURFACE / OUT_SURFACE (e.in / p.out hold surface objects; no fall-back when declined).
 cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const PostParams& q, int out_format, cudaStream_t s,
-                                const char** name, bool srtm_in = false, bool r11 = false);
-cudaError_t launch_rcas_h_post(const RcasParams& p, const PostParams& q, int out_format, cudaStream_t s, const char** name);
+                                const char** name, bool srtm_in = false, bool r11 = false, bool surf_in = false, bool surf_out = false);
+cudaError_t launch_rcas_h_post(const RcasParams& p, const PostParams& q, int out_format, cudaStream_t s, const char** name,
+                               bool surf_out = false);
 
 }  // namespace fsr1

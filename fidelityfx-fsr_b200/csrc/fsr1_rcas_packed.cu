@@ -50,6 +50,13 @@ struct FmtHalf {  // RGBA16F, 8 B per pixel
     if (both) *reinterpret_cast<uint4*>(o) = w;
     else *reinterpret_cast<uint2*>(o) = make_uint2(w.x, w.y);
   }
+  // FSR1_FLAG_OUT_SURFACE: the same bytes through the surface object s, one 8-byte store per pixel
+  static __device__ __forceinline__ void store_surf(unsigned long long s, int x, int y, __half2 oR, __half2 oG, __half2 oB, uint32_t a,
+                                                    bool both) {
+    const uint4 w = pack_pair_half(oR, oG, oB, a);
+    surf_store8(s, x, y, make_uint2(w.x, w.y));
+    if (both) surf_store8(s, x + 1, y, make_uint2(w.z, w.w));
+  }
 };
 
 template <int kBits> struct FmtUnorm {  // R8G8B8A8_UNORM (8) / R10G10B10A2_UNORM (10), 4 B per pixel
@@ -118,7 +125,8 @@ __device__ __forceinline__ typename FM::Raw load_checked(const RcasParams& p, in
 }
 
 // SO: void = FM's own store; otherwise the display epilogue of fsr1_upscale_post (post_pair, fsr1_post.cuh) with its store.
-template <typename FM, bool kChecked, bool kClamp, int kOpt, typename SO = void>
+// kSurfOut (FSR1_FLAG_OUT_SURFACE, FmtHalf only): p.out.base is a surface object; each pixel is one surface store at (x, y).
+template <typename FM, bool kChecked, bool kClamp, int kOpt, typename SO = void, bool kSurfOut = false>
 __device__ __forceinline__ void rcas_rows(const RcasParams& p, int x, int ys, int lane, const PostParams* q = nullptr) {
   constexpr bool kPost = !std::is_void<SO>::value;
   constexpr int kOutBpp = kPost ? PostStore<SO>::kBytes : FM::kBpp;
@@ -163,11 +171,14 @@ __device__ __forceinline__ void rcas_rows(const RcasParams& p, int x, int ys, in
     rcas_pair<kOpt>(prev, d, cur, f, next, sharp, oR, oG, oB);
     if constexpr (kPost) {
       if (writer)
-        post_pair<SO>(*q, pc, dst + (long long)r * p.out.pitch, x, y, oR, oG, oB, (kOpt & kRcasAlpha) ? alphas[r] : FM::opaque(),
-                      !kChecked || x + 1 < p.out.w);
+        post_pair<SO, kSurfOut>(*q, pc, kSurfOut ? p.out.base : dst + (long long)r * p.out.pitch, x, y, oR, oG, oB,
+                                (kOpt & kRcasAlpha) ? alphas[r] : FM::opaque(), !kChecked || x + 1 < p.out.w);
       pc.next_row(*q);
     } else if (writer) {
-      FM::store(dst + (long long)r * p.out.pitch, oR, oG, oB, (kOpt & kRcasAlpha) ? alphas[r] : FM::opaque(), !kChecked || x + 1 < p.out.w);
+      if constexpr (kSurfOut)
+        FM::store_surf(surf_of(p.out), x, y, oR, oG, oB, (kOpt & kRcasAlpha) ? alphas[r] : FM::opaque(), !kChecked || x + 1 < p.out.w);
+      else
+        FM::store(dst + (long long)r * p.out.pitch, oR, oG, oB, (kOpt & kRcasAlpha) ? alphas[r] : FM::opaque(), !kChecked || x + 1 < p.out.w);
     }
   }
 }
@@ -199,6 +210,22 @@ __global__ void __launch_bounds__(32 * kNW) rcas_post_kernel(const RcasParams p,
     rcas_rows<FmtHalf, false, kClamp, kOpt, SO>(p, x, ys, lane, &q);
   else
     rcas_rows<FmtHalf, true, kClamp, kOpt, SO>(p, x, ys, lane, &q);
+}
+
+// FSR1_FLAG_OUT_SURFACE: the two kernels above writing p.out through a surface object (SO = void: rcas_packed_kernel<FmtHalf, ...>)
+template <bool kClamp, int kOpt, typename SO>
+__global__ void __launch_bounds__(32 * kNW) rcas_surf_out_kernel(const RcasParams p, const __grid_constant__ PostParams q) {
+  constexpr bool kPost = !std::is_void<SO>::value;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int x0 = blockIdx.x * kSpan - 2;
+  const int x = x0 + lane * 2;
+  const int ys = p.y0 + (blockIdx.y * kNW + warp) * kRows;
+  if (ys >= p.y1) return;  // whole warp
+  const bool interior = x0 >= 0 && x0 + 64 <= p.in.w && ys >= 1 && ys + kRows < p.in.h && ys + kRows <= p.y1;
+  if (interior)
+    rcas_rows<FmtHalf, false, kClamp, kOpt, SO, true>(p, x, ys, lane, kPost ? &q : nullptr);
+  else
+    rcas_rows<FmtHalf, true, kClamp, kOpt, SO, true>(p, x, ys, lane, kPost ? &q : nullptr);
 }
 
 #ifndef FSR1_CPU_EMU  // tests/emu compiles the device code above for the host and supplies its own launcher
@@ -239,6 +266,19 @@ cudaError_t launch_rcas_u_packed(const RcasParams& p, int format, cudaStream_t s
 }
 
 template <typename SO, bool kClamp>
+static void launch_surf_opt(const RcasParams& p, const PostParams& q, dim3 grid, cudaStream_t s) {
+  switch (p.options & 7) {
+    case 0: rcas_surf_out_kernel<kClamp, 0, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 1: rcas_surf_out_kernel<kClamp, 1, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 2: rcas_surf_out_kernel<kClamp, 2, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 3: rcas_surf_out_kernel<kClamp, 3, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 4: rcas_surf_out_kernel<kClamp, 4, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 5: rcas_surf_out_kernel<kClamp, 5, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    case 6: rcas_surf_out_kernel<kClamp, 6, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+    default: rcas_surf_out_kernel<kClamp, 7, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
+  }
+}
+template <typename SO, bool kClamp>
 static void launch_post_opt(const RcasParams& p, const PostParams& q, dim3 grid, cudaStream_t s) {
   switch (p.options & 7) {
     case 0: rcas_post_kernel<kClamp, 0, SO><<<grid, 32 * kNW, 0, s>>>(p, q); break;
@@ -258,22 +298,42 @@ static cudaError_t launch_post_fmt(const RcasParams& p, const PostParams& q, cud
   else launch_post_opt<SO, false>(p, q, grid, s);
   return cudaGetLastError();
 }
+template <typename SO>
+static cudaError_t launch_surf_fmt(const RcasParams& p, const PostParams& q, cudaStream_t s) {
+  const dim3 grid((p.out.w + kSpan - 1) / kSpan, (p.y1 - p.y0 + kNW * kRows - 1) / (kNW * kRows), 1);
+  if (p.clamp) launch_surf_opt<SO, true>(p, q, grid, s);
+  else launch_surf_opt<SO, false>(p, q, grid, s);
+  return cudaGetLastError();
+}
+// 16-byte aligned input (and output, unless it is a surface): the 128-bit pair loads and stores
+static bool aligned16(const RcasParams& p, bool surf_out, int out_align = 16) {
+  return !((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15) ||
+           (!surf_out && ((reinterpret_cast<uintptr_t>(p.out.base) & (out_align - 1)) || (p.out.pitch & (out_align - 1)))));
+}
 
 // p.in: the RGBA16F intermediate; p.out: RGBA16F (out_format 1), RGBA8_UNORM (3) or RGB10A2_UNORM (4)
-cudaError_t launch_rcas_h_post(const RcasParams& p, const PostParams& q, int out_format, cudaStream_t s, const char** name) {
-  const int oa = out_format == 1 ? 16 : 8;
-  if ((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15) || (reinterpret_cast<uintptr_t>(p.out.base) & (oa - 1)) ||
-      (p.out.pitch & (oa - 1)))
-    return cudaErrorNotSupported;
+cudaError_t launch_rcas_h_post(const RcasParams& p, const PostParams& q, int out_format, cudaStream_t s, const char** name, bool surf_out) {
+  if (!aligned16(p, surf_out, out_format == 1 ? 16 : 8)) return cudaErrorNotSupported;
   switch (out_format) {
-    case 1: *name = "rcas_h_packed_post<2px,4rows,shfl60,rgba16f>"; return launch_post_fmt<__half>(p, q, s);
-    case 3: *name = "rcas_h_packed_post<2px,4rows,shfl60,rgba8>"; return launch_post_fmt<Unorm8>(p, q, s);
-    case 4: *name = "rcas_h_packed_post<2px,4rows,shfl60,rgb10a2>"; return launch_post_fmt<Unorm10>(p, q, s);
+    case 1:
+      *name = surf_out ? "rcas_h_packed_post<2px,4rows,shfl60,rgba16f,surf_out>" : "rcas_h_packed_post<2px,4rows,shfl60,rgba16f>";
+      return surf_out ? launch_surf_fmt<__half>(p, q, s) : launch_post_fmt<__half>(p, q, s);
+    case 3:
+      *name = surf_out ? "rcas_h_packed_post<2px,4rows,shfl60,rgba8,surf_out>" : "rcas_h_packed_post<2px,4rows,shfl60,rgba8>";
+      return surf_out ? launch_surf_fmt<Unorm8>(p, q, s) : launch_post_fmt<Unorm8>(p, q, s);
+    case 4:
+      *name = surf_out ? "rcas_h_packed_post<2px,4rows,shfl60,rgb10a2,surf_out>" : "rcas_h_packed_post<2px,4rows,shfl60,rgb10a2>";
+      return surf_out ? launch_surf_fmt<Unorm10>(p, q, s) : launch_post_fmt<Unorm10>(p, q, s);
   }
   return cudaErrorNotSupported;
 }
 
-cudaError_t launch_rcas_h_packed(const RcasParams& p, cudaStream_t s, const char** name) {
+cudaError_t launch_rcas_h_packed(const RcasParams& p, cudaStream_t s, const char** name, bool surf_out) {
+  if (surf_out) {
+    if (!aligned16(p, true)) return cudaErrorNotSupported;
+    *name = "rcas_h_packed<2px,4rows,shfl60,surf_out>";
+    return launch_surf_fmt<void>(p, PostParams{}, s);
+  }
   if (!aligned(p, 16)) return cudaErrorNotSupported;
   *name = "rcas_h_packed<2px,4rows,shfl60>";
   return launch_fmt<FmtHalf>(p, s);

@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame, fsr1_shard_create_post / fsr1_shard_post, FSR1_FORMAT_R11G11B10_FLOAT */
+#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame, fsr1_shard_create_post / fsr1_shard_post, FSR1_FORMAT_R11G11B10_FLOAT, FSR1_FLAG_IN_SURFACE / FSR1_FLAG_OUT_SURFACE */
 
 enum {
   FSR1_OK = 0,
@@ -109,7 +109,9 @@ enum {
                                        format, EXACT / FORCE_DIRECT / H_REFERENCE / PRECISE, an input (or EASU output) whose base or pitch
                                        is not 16-byte aligned, or constants that do not upscale (0 < con0.x, con0.y <= 1).
                                        fsr1_rcas: FSR1_ERR_INVALID_ARGUMENT. */
-  FSR1_FLAG_H_REFERENCE = 1u << 4   /* fp16 images only: the literal FsrEasuH / FsrRcasH arithmetic (packed-half
+  FSR1_FLAG_IN_SURFACE = 1u << 12,  /* `in` is a CUDA surface object on a 2D CUDA array (EASU's load stage); see "surface images" */
+  FSR1_FLAG_OUT_SURFACE = 1u << 13, /* `out` is a CUDA surface object on a 2D CUDA array (the store of the pass that writes `out`) */
+  FSR1_FLAG_H_REFERENCE = 1u << 4  /* fp16 images only: the literal FsrEasuH / FsrRcasH arithmetic (packed-half
                                        algorithm, half magic numbers, per-operation half rounding), bit-identical
                                        to the reference's H source; a parity path, slower and LESS accurate than
                                        the default fp16 kernels (see DESIGN.md "numerics")                  */
@@ -127,6 +129,31 @@ typedef struct fsr1_image {
   uint32_t format;
   uint32_t reserved;
 } fsr1_image;
+
+/* Surface images (FSR1_FLAG_IN_SURFACE, FSR1_FLAG_OUT_SURFACE): the render target and the display image of an engine, imported through
+ * CUDA interop as CUDA arrays (cudaImportExternalMemory -> cudaExternalMemoryGetMappedMipmappedArray -> level 0), read and written in
+ * place instead of through linear copies.  `data` holds the cudaSurfaceObject_t (cast to a pointer), pitch_bytes is 0, row0 = 0 and
+ * rows = height: a surface image is never a window.  width x height is its logical size, the TOP-LEFT region of the array, which may be
+ * larger; EASU clamps its taps at the logical edge and no kernel touches the array outside [0, width) x [0, height) (the surfaces are
+ * accessed in zero / ignore mode, never trap).  The array must be 2D (not layered, not 3D), created with surface load/store
+ * (cudaArraySurfaceLoadStore), with an element of the format's size: 8 bytes for RGBA16F, 4 for RGBA8_UNORM and RGB10A2_UNORM.  The
+ * bytes stored are exactly those the call stores into a linear image, and every result is bit-identical to the same call on linear
+ * images holding the same pixels; the channel description is the caller's business.
+ *   FSR1_FLAG_IN_SURFACE   `in` is a surface image, RGBA16F only: EASU's load stage of fsr1_easu, fsr1_upscale (fused, or EASU -> tmp
+ *                          -> RCAS), fsr1_upscale_post and fsr1_context_upscale / _render / _post (`in_dev` is the handle, `in_pitch`
+ *                          0).  With FSR1_FLAG_SRTM_INPUT too.  fsr1_rcas: FSR1_ERR_UNSUPPORTED.
+ *   FSR1_FLAG_OUT_SURFACE  `out` is a surface image written by the pass that writes `out`: fsr1_rcas, fsr1_upscale (not with
+ *                          FSR1_FLAG_NO_RCAS), fsr1_upscale_post into RGBA16F, or with TEPD8 / TEPD10 RGBA8_UNORM / RGB10A2_UNORM, and the
+ *                          context calls (`out_dev` is the handle, `out_pitch` 0).  With the RCAS options.  fsr1_easu:
+ *                          FSR1_ERR_UNSUPPORTED.
+ * Images the library owns, and `tmp`, stay linear.  A frame the linear call runs on the fused kernel runs on the fused kernel's surface
+ * twin.  FSR1_ERR_UNSUPPORTED, with nothing launched: another input format, an output format the RGBA16F kernels do not write,
+ * FSR1_FLAG_EXACT / FORCE_DIRECT / H_REFERENCE / PRECISE / RCAS_HX2, constants that do not upscale with FSR1_FLAG_IN_SURFACE, and
+ * fsr1_context_upscale_host, fsr1_shard_create and fsr1_shard_create_post with either flag.  Validation, before any launch and
+ * allocating nothing: first the flag, format and layout rules above (no CUDA call; FSR1_ERR_INVALID_ARGUMENT for a null handle, a
+ * pitch other than 0 or a window), then the array behind each handle (cudaGetSurfaceObjectResourceDesc, cudaArrayGetInfo): an unknown
+ * handle or an extent smaller than width x height returns FSR1_ERR_INVALID_ARGUMENT; a resource that is not a 2D array, or an element
+ * size other than the format's, FSR1_ERR_UNSUPPORTED. */
 
 /* EASU over output rows [y0, y1) (y1 == 0 means "to the last row").  con = con0..con3, 16 words.  in and out have the same format, but
  * for R11G11B10_FLOAT input, whose output is RGBA16F. */
