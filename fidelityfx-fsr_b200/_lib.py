@@ -26,7 +26,7 @@ SYMBOLS = ["fsr1_easu", "fsr1_rcas", "fsr1_easu_input_rows", "fsr1_upscale", "fs
            "fsr1_shard_create", "fsr1_shard_destroy", "fsr1_shard_geometry", "fsr1_shard_export", "fsr1_shard_attach",
            "fsr1_shard_attach_local", "fsr1_shard_input", "fsr1_shard_window", "fsr1_shard_output", "fsr1_shard_arena",
            "fsr1_shard_frame", "fsr1_shard_submit", "fsr1_shard_wait", "fsr1_shard_status", "fsr1_shard_trace",
-           "fsr1_shard_create_post", "fsr1_shard_post"]
+           "fsr1_shard_create_post", "fsr1_shard_post", "fsr1_rcas_post"]
 
 
 class Image(ctypes.Structure):
@@ -74,6 +74,7 @@ def lib():
     postp = ctypes.POINTER(Post)
     L.fsr1_upscale_post.argtypes = [imgp, imgp, imgp, u32p, u32p, postp, u32, u32, u32, vp]
     L.fsr1_context_upscale_post.argtypes = [vp, vp, u64, u32, u32, vp, u64, f32, postp, u32, vp]
+    L.fsr1_rcas_post.argtypes = [imgp, imgp, u32p, postp, u32, u32, u32, vp]
     L.fsr1_context_create.argtypes = [ctypes.POINTER(vp), u32, u32, u32, u32, u32]
     L.fsr1_context_destroy.argtypes = [vp]
     L.fsr1_context_destroy.restype = None

@@ -139,6 +139,19 @@ def upscale_post(inp, tmp, out, econ, rcon, srtm_inverse=False, grain=None, amou
     del keep
 
 
+def rcas_post(inp, out, rcon, srtm_inverse=False, grain=None, amount=0.0, tepd_bits=0, dither=None, frame=0, y0=0, y1=0, flags=0,
+              stream=None):
+    """fsr1_rcas_post: a frame rendered at display size, sharpened straight to the display output in one kernel.  The bits of
+    rcas() on the RGBA16F image of `inp` (through srtm() first with FLAG_SRTM_INPUT), then srtm(inverse), lfga and tepd as in
+    upscale_post().  `inp` is float16 [H,W,4], or int32 [H,W] R11G11B10F codes described by image(t, format=FORMAT_R11G11B10_FLOAT);
+    `out` as upscale_post(), or a surface_image() with FLAG_OUT_SURFACE."""
+    a, b = _as_img(inp), _as_img(out)
+    post, keep = _post(srtm_inverse, grain, amount, tepd_bits, dither, frame)
+    _lib.check(_lib.lib().fsr1_rcas_post(ctypes.byref(a), ctypes.byref(b), (ctypes.c_uint32 * 4)(*rcon), ctypes.byref(post), y0, y1, flags,
+                                         _stream(stream)))
+    del keep
+
+
 def srtm(inp, out, inverse=False, y0=0, y1=0, stream=None):
     """FsrSrtmF / FsrSrtmInvF (ffx_fsr1.h:1044,1046) over rows [y0,y1); `out` may be `inp` (in place)."""
     a, b = _as_img(inp), _as_img(out)

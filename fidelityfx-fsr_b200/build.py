@@ -12,7 +12,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = [os.path.join(HERE, "csrc", f) for f in
-       ("fsr1_direct.cu", "fsr1_easu_tiled.cu", "fsr1_easu_f32.cu", "fsr1_rcas_packed.cu", "fsr1_rcas_f32.cu", "fsr1_href.cu", "fsr1_hx2.cu", "fsr1_pointwise.cu", "fsr1_shard.cu", "fsr1_fused.cu", "fsr1_capi.cu")]
+       ("fsr1_direct.cu", "fsr1_easu_tiled.cu", "fsr1_easu_f32.cu", "fsr1_rcas_packed.cu", "fsr1_rcas_in.cu", "fsr1_rcas_f32.cu", "fsr1_href.cu", "fsr1_hx2.cu", "fsr1_pointwise.cu", "fsr1_shard.cu", "fsr1_fused.cu", "fsr1_capi.cu")]
 DEPS = SRC + [os.path.join(HERE, "csrc", "fsr1_common.cuh"), os.path.join(HERE, "csrc", "fsr1_easu_common.cuh"), os.path.join(HERE, "csrc", "fsr1_easu_quad.cuh"), os.path.join(HERE, "csrc", "fsr1_rcas_math.cuh"), os.path.join(HERE, "csrc", "fsr1_post.cuh"), os.path.join(HERE, "csrc", "fsr1_r11.cuh"),
               os.path.join(HERE, "..", "include", "fsr1_b200.h"),
               os.path.join(HERE, "..", "include", "fsr1_host.h"), os.path.abspath(__file__)]  # this file: the flags

@@ -188,6 +188,21 @@ int srtm_input_check(const fsr1_image* in, const fsr1_image* out, const uint32_t
   return FSR1_OK;
 }
 
+// The images of an RCAS pass over rows [y0, y1) (y1 == 0 becomes the last row): the same logical size, a row range inside the image,
+// windows that hold the rows written and the rows read, linear storage that does not overlap; then the array behind a surface output
+// (the only CUDA call).  fsr1_rcas and fsr1_rcas_post.
+int rcas_images(const fsr1_image* in, const fsr1_image* out, uint32_t y0, uint32_t& y1, bool surf_out) {
+  if (in->width != out->width || in->height != out->height) return FSR1_ERR_INVALID_ARGUMENT;
+  if (y1 == 0) y1 = out->height;
+  if (y0 >= y1 || y1 > out->height) return FSR1_ERR_INVALID_ARGUMENT;
+  if (!window_holds(out, (int)y0, (int)y1 - 1)) return FSR1_ERR_WINDOW;
+  const Rows need = easu_rows(y0, y1, out->height);
+  if (!window_holds(in, (int)need.a, (int)need.b - 1)) return FSR1_ERR_WINDOW;
+  if (!surf_out && overlaps(in, out)) return FSR1_ERR_INVALID_ARGUMENT;
+  if (surf_out) return surface_fits(out);
+  return FSR1_OK;
+}
+
 // the Sample.x hook: `c *= c` in place on the rows the last pass wrote (a separate streaming pass)
 int square_rows(const fsr1_image* img, uint32_t y0, uint32_t y1, cudaStream_t s) {
   const ImgView v = view_of(img);
@@ -510,14 +525,7 @@ int fsr1_rcas(const fsr1_image* in, const fsr1_image* out, const uint32_t con[4]
   if (flags & FSR1_FLAG_IN_SURFACE) return FSR1_ERR_UNSUPPORTED;      // RCAS reads the linear intermediate
   if (surf_out && ((flags & kSurfRefused) || out->format != FSR1_FORMAT_RGBA16F)) return FSR1_ERR_UNSUPPORTED;
   if (in->format != out->format || in->format == FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
-  if (in->width != out->width || in->height != out->height) return FSR1_ERR_INVALID_ARGUMENT;
-  if (y1 == 0) y1 = out->height;
-  if (y0 >= y1 || y1 > out->height) return FSR1_ERR_INVALID_ARGUMENT;
-  if (!window_holds(out, (int)y0, (int)y1 - 1)) return FSR1_ERR_WINDOW;
-  const Rows need = easu_rows(y0, y1, out->height);
-  if (!window_holds(in, (int)need.a, (int)need.b - 1)) return FSR1_ERR_WINDOW;
-  if (!surf_out && overlaps(in, out)) return FSR1_ERR_INVALID_ARGUMENT;
-  if (surf_out && (rc = surface_fits(out)) != FSR1_OK) return rc;
+  if ((rc = rcas_images(in, out, y0, y1, surf_out)) != FSR1_OK) return rc;
 
   RcasParams p = rcas_params(in, out, con, y0, y1, flags);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -563,6 +571,43 @@ int fsr1_upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
 int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, const uint32_t easu_con[16],
                       const uint32_t rcas_con[4], const fsr1_post* post, uint32_t y0, uint32_t y1, uint32_t flags, void* stream) {
   return upscale_post(in, tmp, out, easu_con, rcas_con, post, y0, y1, flags, stream, nullptr, nullptr);
+}
+
+// A frame rendered at display size: one RCAS kernel with the input stage (R11G11B10F decode, FsrSrtmF) and the display epilogue.
+// RGBA16F input without SRTM_INPUT runs the kernels of fsr1_rcas (no ops) and of fsr1_upscale_post's RCAS pass.
+int fsr1_rcas_post(const fsr1_image* in, const fsr1_image* out, const uint32_t rcas_con[4], const fsr1_post* post, uint32_t y0, uint32_t y1,
+                   uint32_t flags, void* stream) {
+  NvtxRange range("RCAS post");
+  // the other arithmetic paths, EASU-only frames and input surfaces: only the packed RGBA16F kernel has the input stage
+  constexpr uint32_t kRefused = FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_HX2 |
+                                FSR1_FLAG_NO_RCAS | FSR1_FLAG_IN_SURFACE;
+  int rc;
+  const bool surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
+  if ((rc = check_image(in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
+  if (!rcas_con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
+  if (flags & kRefused) return FSR1_ERR_UNSUPPORTED;
+  if (in->format != FSR1_FORMAT_RGBA16F && in->format != FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
+  const bool ops = post && post->ops;
+  PostParams q;
+  if (ops && (rc = post_params(post, in->format, out->format, flags, q)) != FSR1_OK) return rc;
+  if (!ops && out->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;
+  const bool r11 = in->format == FSR1_FORMAT_R11G11B10_FLOAT, srtm = (flags & FSR1_FLAG_SRTM_INPUT) != 0;
+  const uint64_t in_align = r11 ? 8 : 16, out_align = out->format == FSR1_FORMAT_RGBA16F ? 16 : 8;  // one vector access per pixel pair
+  if (((uintptr_t)in->data & (in_align - 1)) || (in->pitch_bytes & (in_align - 1))) return FSR1_ERR_UNSUPPORTED;
+  if (!surf_out && (((uintptr_t)out->data & (out_align - 1)) || (out->pitch_bytes & (out_align - 1)))) return FSR1_ERR_UNSUPPORTED;
+  if ((rc = rcas_images(in, out, y0, y1, surf_out)) != FSR1_OK) return rc;
+
+  RcasParams p = rcas_params(in, out, rcas_con, y0, y1, flags);
+  p.options |= (flags & FSR1_FLAG_OUTPUT_SQUARE) ? 4 : 0;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const char* name = "";
+  cudaError_t e;
+  if (r11 || srtm) e = launch_rcas_h_in(p, ops ? &q : nullptr, (int)out->format, r11, srtm, s, &name, surf_out);
+  else if (ops) e = launch_rcas_h_post(p, q, (int)out->format, s, &name, surf_out);
+  else e = launch_rcas_h_packed(p, s, &name, surf_out);
+  if (e != cudaSuccess) return e == cudaErrorNotSupported ? FSR1_ERR_UNSUPPORTED : cuda_fail(e);
+  launched(name);
+  return FSR1_OK;
 }
 
 // ---- pointwise companions ------------------------------------------------------------------------------

@@ -241,5 +241,9 @@ cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const Po
                                 const char** name, bool srtm_in = false, bool r11 = false, bool surf_in = false, bool surf_out = false);
 cudaError_t launch_rcas_h_post(const RcasParams& p, const PostParams& q, int out_format, cudaStream_t s, const char** name,
                                bool surf_out = false);
+// fsr1_rcas_post's input stage: p.in is R11G11B10_FLOAT (r11, 8-byte aligned) or RGBA16F (16-byte aligned), read through FsrSrtmF with
+// srtm; then RCAS and the RGBA16F store (q null) or the epilogue q into out_format.  The rest as launch_rcas_h_post.
+cudaError_t launch_rcas_h_in(const RcasParams& p, const PostParams* q, int out_format, bool r11, bool srtm, cudaStream_t s, const char** name,
+                             bool surf_out = false);
 
 }  // namespace fsr1

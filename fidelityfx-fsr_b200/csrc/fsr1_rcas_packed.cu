@@ -27,6 +27,7 @@ constexpr int kSpan = 60;  // output pixels per warp per row (lanes 1..30)
 // ---- storage formats: how a lane's two pixels are fetched, decoded, encoded and stored --------------------------------
 struct FmtHalf {  // RGBA16F, 8 B per pixel
   static constexpr int kBpp = 8;
+  static constexpr bool kClampArg = false;  // RCAS_CLAMP is the kernel's template bit (InStage, fsr1_rcas_in.cu: p.clamp)
   typedef uint4 Raw;
   static __device__ __forceinline__ Raw zero() { return make_uint4(0u, 0u, 0u, 0u); }
   static __device__ __forceinline__ Raw load2(const unsigned char* a) { return __ldg(reinterpret_cast<const uint4*>(a)); }
@@ -61,6 +62,7 @@ struct FmtHalf {  // RGBA16F, 8 B per pixel
 
 template <int kBits> struct FmtUnorm {  // R8G8B8A8_UNORM (8) / R10G10B10A2_UNORM (10), 4 B per pixel
   static constexpr int kBpp = 4;
+  static constexpr bool kClampArg = false;
   typedef uint2 Raw;
   static __device__ __forceinline__ Raw zero() { return make_uint2(0u, 0u); }
   static __device__ __forceinline__ Raw load2(const unsigned char* a) { return __ldg(reinterpret_cast<const uint2*>(a)); }
@@ -111,23 +113,33 @@ template <int kBits> struct FmtUnorm {  // R8G8B8A8_UNORM (8) / R10G10B10A2_UNOR
   }
 };
 
-// Pixels (x, x+1) of logical row y with the out-of-image rule applied (0, or clamp with kClamp).  Rows outside the STORED
-// window are never used (they are prefetched past the row range of a slab) and read as 0.
+// IN = FM: the pair as loaded; otherwise IN's input stage (InStage, fsr1_rcas_in.cu) turns it into FM's (FmtHalf's) texels
+template <typename FM, typename IN>
+__device__ __forceinline__ typename FM::Raw in_texels(typename IN::Raw v, bool srtm) {
+  if constexpr (std::is_same<FM, IN>::value) return v;
+  else return IN::texels(v, srtm);
+}
+
+// Pixels (x, x+1) of logical row y with the out-of-image rule applied (0, or clamp with kClamp, or with p.clamp for FM::kClampArg).
+// Rows outside the STORED window are never used (they are prefetched past the row range of a slab) and read as 0.
 template <typename FM, bool kClamp>
 __device__ __forceinline__ typename FM::Raw load_checked(const RcasParams& p, int x, int y) {
-  if (kClamp) y = clampi(y, 0, p.in.h - 1);
+  const bool clamp = kClamp || (FM::kClampArg && p.clamp);
+  if (clamp) y = clampi(y, 0, p.in.h - 1);
   if (!row_stored(p.in, y)) return FM::zero();
   const unsigned char* row = p.in.base + (long long)(y - p.in.row0) * p.in.pitch;
   if (x >= 0 && x + 1 < p.in.w) return FM::load2(row + (long long)x * FM::kBpp);
-  if (kClamp) return FM::load11(row + (long long)clampi(x, 0, p.in.w - 1) * FM::kBpp, row + (long long)clampi(x + 1, 0, p.in.w - 1) * FM::kBpp);
+  if (clamp) return FM::load11(row + (long long)clampi(x, 0, p.in.w - 1) * FM::kBpp, row + (long long)clampi(x + 1, 0, p.in.w - 1) * FM::kBpp);
   return FM::load11(x >= 0 && x < p.in.w ? row + (long long)x * FM::kBpp : nullptr,
                     x + 1 >= 0 && x + 1 < p.in.w ? row + (long long)(x + 1) * FM::kBpp : nullptr);
 }
 
 // SO: void = FM's own store; otherwise the display epilogue of fsr1_upscale_post (post_pair, fsr1_post.cuh) with its store.
 // kSurfOut (FSR1_FLAG_OUT_SURFACE, FmtHalf only): p.out.base is a surface object; each pixel is one surface store at (x, y).
-template <typename FM, bool kChecked, bool kClamp, int kOpt, typename SO = void, bool kSurfOut = false>
-__device__ __forceinline__ void rcas_rows(const RcasParams& p, int x, int ys, int lane, const PostParams* q = nullptr) {
+// IN (FM = FmtHalf only): the input stage of fsr1_rcas_post (InStage, fsr1_rcas_in.cu), which reads p.in in its own format; srtm is
+// its argument.
+template <typename FM, bool kChecked, bool kClamp, int kOpt, typename SO = void, bool kSurfOut = false, typename IN = FM>
+__device__ __forceinline__ void rcas_rows(const RcasParams& p, int x, int ys, int lane, const PostParams* q = nullptr, bool srtm = false) {
   constexpr bool kPost = !std::is_void<SO>::value;
   constexpr int kOutBpp = kPost ? PostStore<SO>::kBytes : FM::kBpp;
   const __half2 sharp = uh2(p.sharp_h2);
@@ -136,17 +148,17 @@ __device__ __forceinline__ void rcas_rows(const RcasParams& p, int x, int ys, in
   Row3 rows[kRows + 2];
   uint32_t alphas[kRows];  // kRcasAlpha only: the centre pixels' alpha
   if (!kChecked) {  // one 64-bit address, then += pitch: no per-row address arithmetic
-    const unsigned char* src = p.in.base + (long long)(ys - 1 - p.in.row0) * p.in.pitch + (long long)x * FM::kBpp;
+    const unsigned char* src = p.in.base + (long long)(ys - 1 - p.in.row0) * p.in.pitch + (long long)x * IN::kBpp;
 #pragma unroll
     for (int r = 0; r < kRows + 2; r++) {
-      const typename FM::Raw v = FM::load2(src + (long long)r * p.in.pitch);
+      const typename FM::Raw v = in_texels<FM, IN>(IN::load2(src + (long long)r * p.in.pitch), srtm);
       rows[r] = FM::decode(v);
       if ((kOpt & kRcasAlpha) && r >= 1 && r <= kRows) alphas[r - 1] = FM::alpha(v);
     }
   } else {
 #pragma unroll
     for (int r = 0; r < kRows + 2; r++) {
-      const typename FM::Raw v = load_checked<FM, kClamp>(p, x, ys - 1 + r);
+      const typename FM::Raw v = in_texels<FM, IN>(load_checked<IN, kClamp>(p, x, ys - 1 + r), srtm);
       rows[r] = FM::decode(v);
       if ((kOpt & kRcasAlpha) && r >= 1 && r <= kRows) alphas[r - 1] = FM::alpha(v);
     }
@@ -228,7 +240,8 @@ __global__ void __launch_bounds__(32 * kNW) rcas_surf_out_kernel(const RcasParam
     rcas_rows<FmtHalf, true, kClamp, kOpt, SO, true>(p, x, ys, lane, kPost ? &q : nullptr);
 }
 
-#ifndef FSR1_CPU_EMU  // tests/emu compiles the device code above for the host and supplies its own launcher
+// tests/emu compiles the device code above for the host and supplies its own launcher; fsr1_rcas_in.cu takes the templates only
+#if !defined(FSR1_CPU_EMU) && !defined(FSR1_RCAS_PACKED_TEMPLATES_ONLY)
 template <typename FM, bool kClamp>
 static void launch_opt(const RcasParams& p, dim3 grid, cudaStream_t s) {
   switch (p.options & 7) {

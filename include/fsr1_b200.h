@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame, fsr1_shard_create_post / fsr1_shard_post, FSR1_FORMAT_R11G11B10_FLOAT, FSR1_FLAG_IN_SURFACE / FSR1_FLAG_OUT_SURFACE */
+#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame, fsr1_shard_create_post / fsr1_shard_post, FSR1_FORMAT_R11G11B10_FLOAT, FSR1_FLAG_IN_SURFACE / FSR1_FLAG_OUT_SURFACE, fsr1_rcas_post */
 
 enum {
   FSR1_OK = 0,
@@ -341,6 +341,28 @@ int fsr1_upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_im
 int fsr1_context_upscale_post(fsr1_context* ctx, const void* in_dev, uint64_t in_pitch, uint32_t render_width,
                               uint32_t render_height, void* out_dev, uint64_t out_pitch, float sharpness_stops,
                               const fsr1_post* post, uint32_t flags, void* stream);
+
+/* Sharpen a frame rendered at display resolution (render size = display size: a native / "sharpen only" setting, dynamic resolution
+ * at 100 %) straight to the display output: the input stage, RCAS and the display steps of fsr1_upscale_post in ONE kernel, with no
+ * EASU pass and no intermediate.  On rows [y0, y1) (y1 == 0: to the last row) the result is bit-identical to
+ *     I = in (RGBA16F), or for R11G11B10_FLOAT the RGBA16F image (R, G, B, 1.0) of its codes
+ *     FSR1_FLAG_SRTM_INPUT:  I = fsr1_srtm(I, ., 0) over the rows RCAS reads, [y0-1, y1+1) clipped to the image
+ *     fsr1_rcas(I, T, rcas_con, y0, y1, the RCAS_CLAMP / RCAS_DENOISE / RCAS_PASSTHROUGH_ALPHA / OUTPUT_SQUARE bits of flags), T RGBA16F
+ *     the steps of `post` on T as fsr1_upscale_post applies them (SRTM inverse, LFGA, TEPD8 / TEPD10), the last one writing `out`.
+ * Out-of-image taps read 0 in the decoded domain (or clamp with RCAS_CLAMP); R11G11B10_FLOAT has no alpha, so PASSTHROUGH_ALPHA gives 1.0.
+ * post == NULL or ops == 0 on RGBA16F input without SRTM_INPUT is exactly fsr1_rcas (the same kernel).
+ *   in      RGBA16F (base and pitch 16-byte aligned) or R11G11B10_FLOAT (8-byte aligned), linear, possibly a row window holding rows
+ *           [y0-1, y1+1) clipped to the image (the rule of fsr1_rcas).
+ *   out     in's logical size; RGBA16F (16-byte aligned), or with TEPD the UNORM format it implies (8-byte aligned), as fsr1_upscale_post;
+ *           a surface image with FSR1_FLAG_OUT_SURFACE.
+ *   flags   RCAS_CLAMP, RCAS_DENOISE, RCAS_PASSTHROUGH_ALPHA, OUTPUT_SQUARE, SRTM_INPUT, OUT_SURFACE; FUSED is accepted and has no effect.
+ * FSR1_ERR_INVALID_ARGUMENT: a null in, out or rcas_con, an unknown flag, a bad row range, in and out of different sizes, linear storage
+ * of in and out that overlaps, and every refusal of fsr1_upscale_post's post description.  FSR1_ERR_UNSUPPORTED: another input or
+ * output format, EXACT / FORCE_DIRECT / H_REFERENCE / PRECISE / RCAS_HX2 / NO_RCAS / IN_SURFACE, or an unaligned layout (there is no
+ * fall-back kernel).  FSR1_ERR_WINDOW: a window that does not hold the rows.  All returned before any CUDA call but the array query of
+ * FSR1_FLAG_OUT_SURFACE. */
+int fsr1_rcas_post(const fsr1_image* in, const fsr1_image* out, const uint32_t rcas_con[4], const fsr1_post* post, uint32_t y0, uint32_t y1,
+                   uint32_t flags, void* stream);
 
 /* Display output from the sharded frame stream: every frame of the shard is fsr1_upscale_post with `post` instead of fsr1_upscale,
  * so each rank's output slab holds the display image's rows (for rows [out_row0, out_row1), bit-identical to the same rows of
