@@ -13,6 +13,7 @@ FLAG_RCAS_CLAMP, FLAG_EXACT, FLAG_FORCE_DIRECT, FLAG_NO_RCAS, FLAG_H_REFERENCE, 
 FLAG_RCAS_DENOISE, FLAG_RCAS_PASSTHROUGH_ALPHA, FLAG_OUTPUT_SQUARE, FLAG_FUSED, FLAG_RCAS_HX2 = 64, 128, 256, 512, 1024
 FLAG_SRTM_INPUT = 2048
 FLAG_IN_SURFACE, FLAG_OUT_SURFACE = 1 << 12, 1 << 13  # `in` / `out` is a CUDA surface object (api.surface_image)
+FLAG_IN_TEXTURE = 1 << 14  # `in` is a CUDA texture object (api.texture_image)
 POST_SRTM_INVERSE, POST_LFGA, POST_TEPD8, POST_TEPD10 = 1, 2, 4, 8
 SHARD_ONE_STREAM, SHARD_SKIP_HALO, SHARD_TRACE, SHARD_HANDLE_BYTES = 1 << 16, 1 << 17, 1 << 18, 64
 SHARD_DYNAMIC = 1 << 19

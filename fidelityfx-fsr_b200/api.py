@@ -10,7 +10,7 @@ import torch
 from . import _lib
 from ._lib import FORMAT_R11G11B10_FLOAT, FORMAT_RGB10A2_UNORM, FORMAT_RGBA8_UNORM  # noqa: F401
 from ._lib import FLAG_FUSED, FLAG_OUTPUT_SQUARE, FLAG_RCAS_HX2, FLAG_SRTM_INPUT  # noqa: F401
-from ._lib import FLAG_IN_SURFACE, FLAG_OUT_SURFACE  # noqa: F401
+from ._lib import FLAG_IN_SURFACE, FLAG_OUT_SURFACE, FLAG_IN_TEXTURE  # noqa: F401
 from ._lib import POST_LFGA, POST_SRTM_INVERSE, POST_TEPD10, POST_TEPD8  # noqa: F401
 from ._lib import (FLAG_EXACT, FLAG_FORCE_DIRECT, FLAG_H_REFERENCE, FLAG_NO_RCAS, FLAG_PRECISE, FLAG_RCAS_DENOISE, FLAG_RCAS_PASSTHROUGH_ALPHA, FLAG_RCAS_CLAMP, FORMAT_RGBA16F,  # noqa: F401
                    FORMAT_RGBA32F, Fsr1Error, Image)
@@ -78,6 +78,15 @@ def surface_image(handle, width, height, format):
     the top-left width x height is the image.  Pitch 0, the whole image (never a window)."""
     if not isinstance(handle, int) or handle <= 0:
         raise Fsr1Error("a surface image is a nonzero cudaSurfaceObject_t handle (int)")
+    return Image(handle, 0, int(width), int(height), 0, int(height), int(format), 0)
+
+
+def texture_image(handle, width, height, format):
+    """A texture image (FLAG_IN_TEXTURE): the CUDA texture object `handle` (an int) on a 2D CUDA array with unsigned-integer channels
+    (16,16,16,16 for FORMAT_RGBA16F, 32 for FORMAT_R11G11B10_FLOAT), point filtering, unnormalized coordinates, element read mode; the
+    top-left width x height of the array is the image.  Pitch 0, the whole image (never a window)."""
+    if not isinstance(handle, int) or handle <= 0:
+        raise Fsr1Error("a texture image is a nonzero cudaTextureObject_t handle (int)")
     return Image(handle, 0, int(width), int(height), 0, int(height), int(format), 0)
 
 
@@ -281,11 +290,12 @@ def launch_count():
 
 
 def _dev(x, flags, flag):
-    """(address, pitch) of a device image argument of the context calls: a tensor, or with `flag` in `flags` a surface object handle
-    (int) with pitch 0."""
+    """(address, pitch) of a device image argument of the context calls: a tensor, or with a bit of `flag` in `flags` a surface or
+    texture object handle (int) with pitch 0."""
     if flags & flag:
         if not isinstance(x, int):
-            raise Fsr1Error("with FLAG_IN_SURFACE / FLAG_OUT_SURFACE the matching image is a surface object handle (int)")
+            raise Fsr1Error("with FLAG_IN_SURFACE / FLAG_IN_TEXTURE / FLAG_OUT_SURFACE the matching image is a surface or texture object "
+                            "handle (int)")
         return ctypes.c_void_p(x), 0
     return ctypes.c_void_p(x.data_ptr()), x.stride(0) * x.element_size()
 
@@ -293,7 +303,8 @@ def _dev(x, flags, flag):
 class HostContext:
     """fsr1_context_*: owns the intermediate and device staging; frames live in (pinned) host memory.
     fmt: the input's format; the output is in it too, but float16 [H, W, 4] (RGBA16F) for FORMAT_R11G11B10_FLOAT input (int32 [H, W]).
-    The device-frame calls take a surface object handle (int) in place of `in_dev` / `out_dev` with FLAG_IN_SURFACE / FLAG_OUT_SURFACE."""
+    The device-frame calls take a surface object handle (int) in place of `in_dev` / `out_dev` with FLAG_IN_SURFACE / FLAG_OUT_SURFACE,
+    and a texture object handle in place of `in_dev` with FLAG_IN_TEXTURE."""
 
     def __init__(self, in_w, in_h, out_w, out_h, fmt=FORMAT_RGBA16F):
         self._h = ctypes.c_void_p()
@@ -307,13 +318,13 @@ class HostContext:
             ctypes.c_float(sharpness), flags, _stream(stream)))
 
     def upscale(self, in_dev, out_dev, sharpness=0.25, flags=0, stream=None):
-        (a, ap), (b, bp) = _dev(in_dev, flags, FLAG_IN_SURFACE), _dev(out_dev, flags, FLAG_OUT_SURFACE)
+        (a, ap), (b, bp) = _dev(in_dev, flags, FLAG_IN_SURFACE | FLAG_IN_TEXTURE), _dev(out_dev, flags, FLAG_OUT_SURFACE)
         _lib.check(_lib.lib().fsr1_context_upscale(self._h, a, ap, b, bp, ctypes.c_float(sharpness), flags, _stream(stream)))
 
     def upscale_render(self, in_dev, render_w, render_h, out_dev, sharpness=0.25, flags=0, stream=None):
         """One frame rendered at render_w x render_h (dynamic resolution): the top-left render region of `in_dev`, upscaled to the
         context's output size with constants rebuilt from this frame's render size."""
-        (a, ap), (b, bp) = _dev(in_dev, flags, FLAG_IN_SURFACE), _dev(out_dev, flags, FLAG_OUT_SURFACE)
+        (a, ap), (b, bp) = _dev(in_dev, flags, FLAG_IN_SURFACE | FLAG_IN_TEXTURE), _dev(out_dev, flags, FLAG_OUT_SURFACE)
         _lib.check(_lib.lib().fsr1_context_upscale_render(self._h, a, ap, render_w, render_h, b, bp, ctypes.c_float(sharpness), flags,
                                                           _stream(stream)))
 
@@ -322,7 +333,7 @@ class HostContext:
         """fsr1_context_upscale_post: upscale_render followed by the display steps of api.upscale_post; `out_dev` is uint8 [H,W,4]
         with tepd_bits 8, int32 [H,W] with 10, float16 [H,W,4] otherwise.  render size 0 = the context's input size."""
         post, keep = _post(srtm_inverse, grain, amount, tepd_bits, dither, frame)
-        (a, ap), (b, bp) = _dev(in_dev, flags, FLAG_IN_SURFACE), _dev(out_dev, flags, FLAG_OUT_SURFACE)
+        (a, ap), (b, bp) = _dev(in_dev, flags, FLAG_IN_SURFACE | FLAG_IN_TEXTURE), _dev(out_dev, flags, FLAG_OUT_SURFACE)
         _lib.check(_lib.lib().fsr1_context_upscale_post(self._h, a, ap, render_w, render_h, b, bp, ctypes.c_float(sharpness),
                                                         ctypes.byref(post), flags, _stream(stream)))
         del keep

@@ -84,21 +84,29 @@ int host_cell(uint32_t o, float scale, float offset) {
 constexpr uint32_t kAllFlags = FSR1_FLAG_RCAS_CLAMP | FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_NO_RCAS |
                                FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_DENOISE |
                                FSR1_FLAG_RCAS_PASSTHROUGH_ALPHA | FSR1_FLAG_OUTPUT_SQUARE | FSR1_FLAG_FUSED | FSR1_FLAG_RCAS_HX2 |
-                               FSR1_FLAG_SRTM_INPUT | FSR1_FLAG_IN_SURFACE | FSR1_FLAG_OUT_SURFACE;
+                               FSR1_FLAG_SRTM_INPUT | FSR1_FLAG_IN_SURFACE | FSR1_FLAG_OUT_SURFACE | FSR1_FLAG_IN_TEXTURE;
 
-// ---- surface images (FSR1_FLAG_IN_SURFACE / FSR1_FLAG_OUT_SURFACE, include/fsr1_b200.h) ------------------------------------------
-constexpr uint32_t kSurfFlags = FSR1_FLAG_IN_SURFACE | FSR1_FLAG_OUT_SURFACE;
-// the surface stages exist in the RGBA16F production kernels only (tiled EASU, packed RCAS, fused, post)
+// ---- array images (FSR1_FLAG_IN_SURFACE / FSR1_FLAG_IN_TEXTURE / FSR1_FLAG_OUT_SURFACE, include/fsr1_b200.h) -----------------------
+constexpr uint32_t kArrayIn = FSR1_FLAG_IN_SURFACE | FSR1_FLAG_IN_TEXTURE;  // `in` is a CUDA array: at most one of them
+constexpr uint32_t kArrayFlags = kArrayIn | FSR1_FLAG_OUT_SURFACE;
+// the array stages exist in the RGBA16F production kernels only (tiled EASU, packed RCAS, fused, post) and their R11G11B10F variants
 constexpr uint32_t kSurfRefused = FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_HX2;
 
-// The layout of a surface image: a handle, pitch 0, the whole image (never a window).  No CUDA call.
-int check_surface(const fsr1_image* im) {
+// flags the call cannot take whatever it is: an unknown bit, or both kinds of array input
+bool bad_flags(uint32_t flags) { return (flags & ~kAllFlags) || (flags & kArrayIn) == kArrayIn; }
+
+// The layout of an array image (a surface or texture image): a handle, pitch 0, the whole image (never a window).  No CUDA call.
+int check_array(const fsr1_image* im) {
   if (!im || !im->data || im->width == 0 || im->height == 0 || im->width > 32768u || im->height > 32768u) return FSR1_ERR_INVALID_ARGUMENT;
   if (!bytes_per_pixel(im->format) || im->pitch_bytes != 0 || im->row0 != 0 || im->rows != im->height) return FSR1_ERR_INVALID_ARGUMENT;
   return FSR1_OK;
 }
-// an image the call reads or writes: a surface image when the flag that describes it is set, a linear one otherwise
-int check_io(const fsr1_image* im, bool surface) { return surface ? check_surface(im) : check_image(im); }
+// an image the call reads or writes: an array image when a flag that describes it is set, a linear one otherwise
+int check_io(const fsr1_image* im, bool array) { return array ? check_array(im) : check_image(im); }
+// where EASU's load stage reads `in` from under `flags`
+InSrc in_src(uint32_t flags) {
+  return (flags & FSR1_FLAG_IN_TEXTURE) ? kInTex : (flags & FSR1_FLAG_IN_SURFACE) ? kInSurf : kInTma;
+}
 
 // The CUDA array behind a surface image: a 2D array (not layered, not 3D) whose element is the format's size and whose extent holds
 // width x height.  An unknown handle: FSR1_ERR_INVALID_ARGUMENT (the failed query's error is cleared: nothing has launched).
@@ -122,13 +130,48 @@ int surface_fits(const fsr1_image* im) {
   return FSR1_OK;
 }
 
-// Every refusal of the surface flags of a call that may take both (fsr1_upscale, fsr1_upscale_post), before anything launches, so that
-// the two-kernel path never runs EASU and then refuses RCAS's store: the flag and format rules first, then the arrays.  unorm_out: the
-// output may also be RGBA8 / RGB10A2 (fsr1_upscale_post's TEPD; its format rules are post_params').  The layouts were checked already.
-int surface_rules(const fsr1_image* in, const fsr1_image* out, const uint32_t* easu_con, uint32_t flags, bool unorm_out) {
+// The texture object behind a texture image: a level-0 2D array resource (not layered, not 3D) whose channels are unsigned integers of
+// the format's layout (16,16,16,16 for RGBA16F, 32 for R11G11B10F), read in element mode at unnormalized coordinates with point
+// filtering and no sRGB decode, so that every fetch returns the texel's raw bits; its extent holds width x height.  An unknown handle or
+// a short extent: FSR1_ERR_INVALID_ARGUMENT (a failed query's error is cleared: nothing has launched); anything else that differs:
+// FSR1_ERR_UNSUPPORTED.  The address mode is free: every fetch is inside the logical image.
+int texture_fits(const fsr1_image* im) {
+  const cudaTextureObject_t t = (cudaTextureObject_t)(uintptr_t)im->data;
+  cudaResourceDesc rd;
+  cudaTextureDesc td;
+  cudaChannelFormatDesc cd;
+  cudaExtent ext;
+  unsigned int aflags = 0;
+  if (cudaGetTextureObjectResourceDesc(&rd, t) != cudaSuccess || cudaGetTextureObjectTextureDesc(&td, t) != cudaSuccess) {
+    cudaGetLastError();
+    return FSR1_ERR_INVALID_ARGUMENT;
+  }
+  if (rd.resType != cudaResourceTypeArray) return FSR1_ERR_UNSUPPORTED;  // pitch2D, linear and mipmapped resources
+  if (td.readMode != cudaReadModeElementType || td.normalizedCoords || td.filterMode != cudaFilterModePoint || td.sRGB)
+    return FSR1_ERR_UNSUPPORTED;
+  if (cudaArrayGetInfo(&cd, &ext, &aflags, rd.res.array.array) != cudaSuccess) {
+    cudaGetLastError();
+    return FSR1_ERR_INVALID_ARGUMENT;
+  }
+  if (ext.depth != 0 || (aflags & cudaArrayLayered)) return FSR1_ERR_UNSUPPORTED;
+  const bool bits = im->format == FSR1_FORMAT_RGBA16F ? cd.x == 16 && cd.y == 16 && cd.z == 16 && cd.w == 16
+                  : im->format == FSR1_FORMAT_R11G11B10_FLOAT && cd.x == 32 && cd.y == 0 && cd.z == 0 && cd.w == 0;
+  if (cd.f != cudaChannelFormatKindUnsigned || !bits) return FSR1_ERR_UNSUPPORTED;  // a float kind would convert, losing the bits
+  if (ext.width < im->width || ext.height < im->height) return FSR1_ERR_INVALID_ARGUMENT;
+  return FSR1_OK;
+}
+// the CUDA array behind an array input
+int in_array_fits(const fsr1_image* in, uint32_t flags) { return (flags & FSR1_FLAG_IN_TEXTURE) ? texture_fits(in) : surface_fits(in); }
+
+// Every refusal of the array flags of a call that may take both sides (fsr1_upscale, fsr1_upscale_post), before anything launches, so
+// that the two-kernel path never runs EASU and then refuses RCAS's store: the flag and format rules first, then the arrays.  unorm_out:
+// the output may also be RGBA8 / RGB10A2 (fsr1_upscale_post's TEPD; its format rules are post_params').  The layouts were checked already.
+int array_rules(const fsr1_image* in, const fsr1_image* out, const uint32_t* easu_con, uint32_t flags, bool unorm_out) {
   if (flags & kSurfRefused) return FSR1_ERR_UNSUPPORTED;
-  if (in->format != FSR1_FORMAT_RGBA16F) return FSR1_ERR_UNSUPPORTED;  // the surface twins are those of the RGBA16F kernels
-  if (flags & FSR1_FLAG_IN_SURFACE) {
+  // the array twins are those of the RGBA16F kernels, and with a texture input those of their R11G11B10F variants
+  const bool tex_r11 = (flags & FSR1_FLAG_IN_TEXTURE) && in->format == FSR1_FORMAT_R11G11B10_FLOAT;
+  if (in->format != FSR1_FORMAT_RGBA16F && !tex_r11) return FSR1_ERR_UNSUPPORTED;
+  if (flags & kArrayIn) {
     if (!is_upscale(word_as_float(easu_con[0]), word_as_float(easu_con[1]))) return FSR1_ERR_UNSUPPORTED;  // no direct kernel reads one
   }
   if (flags & FSR1_FLAG_OUT_SURFACE) {
@@ -138,7 +181,7 @@ int surface_rules(const fsr1_image* in, const fsr1_image* out, const uint32_t* e
     if (!ok) return FSR1_ERR_UNSUPPORTED;
   }
   int rc;
-  if ((flags & FSR1_FLAG_IN_SURFACE) && (rc = surface_fits(in)) != FSR1_OK) return rc;
+  if ((flags & kArrayIn) && (rc = in_array_fits(in, flags)) != FSR1_OK) return rc;
   if ((flags & FSR1_FLAG_OUT_SURFACE) && (rc = surface_fits(out)) != FSR1_OK) return rc;
   return FSR1_OK;
 }
@@ -182,7 +225,7 @@ RcasParams rcas_params(const fsr1_image* in, const fsr1_image* out, const uint32
 int srtm_input_check(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], uint32_t flags) {
   if (in->format != FSR1_FORMAT_RGBA16F && in->format != FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
   if (flags & (FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE)) return FSR1_ERR_UNSUPPORTED;
-  if (!(flags & FSR1_FLAG_IN_SURFACE) && (((uintptr_t)in->data & 15) || (in->pitch_bytes & 15))) return FSR1_ERR_UNSUPPORTED;  // TMA
+  if (!(flags & kArrayIn) && (((uintptr_t)in->data & 15) || (in->pitch_bytes & 15))) return FSR1_ERR_UNSUPPORTED;  // TMA
   if (out && (((uintptr_t)out->data & 15) || (out->pitch_bytes & 15))) return FSR1_ERR_UNSUPPORTED;  // 16-byte pixel-pair stores
   if (!is_upscale(word_as_float(con[0]), word_as_float(con[1]))) return FSR1_ERR_UNSUPPORTED;
   return FSR1_OK;
@@ -253,11 +296,12 @@ cudaError_t launch_fused(const fsr1_image* in, const fsr1_image* out, const uint
   EasuParams p = easu_params(in, out, easu_con, y0, y1);
   if (sync) p.sync = *sync;
   const bool srtm_in = (flags & FSR1_FLAG_SRTM_INPUT) != 0, r11 = in->format == FSR1_FORMAT_R11G11B10_FLOAT;
-  const bool surf_in = (flags & FSR1_FLAG_IN_SURFACE) != 0, surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
+  const InSrc src = in_src(flags);
+  const bool surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const char* name = "";
-  const cudaError_t e = q ? launch_fused_h_post(p, rcas_con[1], *q, (int)out->format, s, &name, srtm_in, r11, surf_in, surf_out)
-                          : launch_fused_h(p, rcas_con[1], 0, s, &name, srtm_in, r11, surf_in, surf_out);
+  const cudaError_t e = q ? launch_fused_h_post(p, rcas_con[1], *q, (int)out->format, s, &name, srtm_in, r11, src, surf_out)
+                          : launch_fused_h(p, rcas_con[1], 0, s, &name, srtm_in, r11, src, surf_out);
   if (e != cudaSuccess) return e;
   launched(name);
   if (sync) *sync_taken = true;
@@ -287,7 +331,7 @@ int post_params(const fsr1_post* post, uint32_t in_format, uint32_t out_format, 
   if (ops & ~kAllPost) return FSR1_ERR_INVALID_ARGUMENT;
   if ((ops & FSR1_POST_TEPD8) && (ops & FSR1_POST_TEPD10)) return FSR1_ERR_INVALID_ARGUMENT;
   if ((ops & FSR1_POST_LFGA) && !post->grain) return FSR1_ERR_INVALID_ARGUMENT;
-  if (flags & ~kAllFlags) return FSR1_ERR_INVALID_ARGUMENT;
+  if (bad_flags(flags)) return FSR1_ERR_INVALID_ARGUMENT;
   int rc;
   const bool tepd = (ops & (FSR1_POST_TEPD8 | FSR1_POST_TEPD10)) != 0;
   if ((rc = post_tile(post->grain, (ops & FSR1_POST_LFGA) != 0, q.grain, q.grain_fmt)) != FSR1_OK) return rc;
@@ -316,14 +360,15 @@ int easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], ui
          const HaloSync* sync, bool* sync_taken) {
   NvtxRange range("EASU");
   int rc;
-  const bool surf_in = (flags & FSR1_FLAG_IN_SURFACE) != 0;
-  if ((rc = check_io(in, surf_in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
-  if (!con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
+  const bool array_in = (flags & kArrayIn) != 0, tex_in = (flags & FSR1_FLAG_IN_TEXTURE) != 0;
+  if ((rc = check_io(in, array_in)) != FSR1_OK || (rc = check_image(out)) != FSR1_OK) return rc;
+  if (!con || bad_flags(flags)) return FSR1_ERR_INVALID_ARGUMENT;
   if (flags & FSR1_FLAG_OUT_SURFACE) return FSR1_ERR_UNSUPPORTED;  // EASU stores to linear images only
-  if (surf_in && (flags & kSurfRefused)) return FSR1_ERR_UNSUPPORTED;
-  if (surf_in && (in->format != FSR1_FORMAT_RGBA16F || !is_upscale(word_as_float(con[0]), word_as_float(con[1])))) return FSR1_ERR_UNSUPPORTED;
-  if (out->format != easu_out_format(in->format)) return FSR1_ERR_UNSUPPORTED;
+  if (array_in && (flags & kSurfRefused)) return FSR1_ERR_UNSUPPORTED;
   const bool r11 = in->format == FSR1_FORMAT_R11G11B10_FLOAT;
+  if (array_in && ((in->format != FSR1_FORMAT_RGBA16F && !(tex_in && r11)) || !is_upscale(word_as_float(con[0]), word_as_float(con[1]))))
+    return FSR1_ERR_UNSUPPORTED;
+  if (out->format != easu_out_format(in->format)) return FSR1_ERR_UNSUPPORTED;
   if (r11 && (flags & kR11Refused)) return FSR1_ERR_UNSUPPORTED;
   if (y1 == 0) y1 = out->height;
   if (y0 >= y1 || y1 > out->height) return FSR1_ERR_INVALID_ARGUMENT;
@@ -333,7 +378,7 @@ int easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], ui
   if (!window_holds(in, (int)r0, (int)r1)) return FSR1_ERR_WINDOW;
   const bool srtm_in = (flags & FSR1_FLAG_SRTM_INPUT) != 0;
   if (srtm_in && (rc = srtm_input_check(in, out, con, flags)) != FSR1_OK) return rc;
-  if (surf_in && (rc = surface_fits(in)) != FSR1_OK) return rc;
+  if (array_in && (rc = in_array_fits(in, flags)) != FSR1_OK) return rc;
 
   EasuParams p = easu_params(in, out, con, y0, y1);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -349,11 +394,11 @@ int easu(const fsr1_image* in, const fsr1_image* out, const uint32_t con[16], ui
     if (flags & FSR1_FLAG_PRECISE) e = launch_easu_h_precise(p, s, &name);
     if (e == cudaErrorNotSupported) {
       if (sync) p.sync = *sync;  // sharded frame: the neighbour hand-shake rides inside the kernel
-      e = launch_easu_h_tiled(p, s, &name, srtm_in, r11, surf_in);
+      e = launch_easu_h_tiled(p, s, &name, srtm_in, r11, in_src(flags));
       if (e == cudaSuccess && sync) *sync_taken = true;
       p.sync = HaloSync{};
     }
-    if (e == cudaErrorNotSupported && (srtm_in || surf_in)) return FSR1_ERR_UNSUPPORTED;  // nothing launched; no other kernel applies the flag
+    if (e == cudaErrorNotSupported && (srtm_in || array_in)) return FSR1_ERR_UNSUPPORTED;  // nothing launched; no other kernel applies the flag
   } else if (in->format == FSR1_FORMAT_RGBA32F && !exact && !(flags & FSR1_FLAG_FORCE_DIRECT)) {
     e = launch_easu_f32_tiled(p, s, &name);
   } else if ((in->format == FSR1_FORMAT_RGBA8_UNORM || in->format == FSR1_FORMAT_RGB10A2_UNORM) && !exact &&
@@ -378,19 +423,19 @@ int upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, 
       return FSR1_ERR_UNSUPPORTED;
     if (flags & kR11Refused) return FSR1_ERR_UNSUPPORTED;
   }
-  const bool surf_in = (flags & FSR1_FLAG_IN_SURFACE) != 0, surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
+  const bool array_in = (flags & kArrayIn) != 0, surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
   int rc;
-  if (surf_in || surf_out) {  // every refusal of the surfaces before anything launches
-    if ((rc = check_io(in, surf_in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
-    if (!easu_con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
-    if ((rc = surface_rules(in, out, easu_con, flags, false)) != FSR1_OK) return rc;
+  if (array_in || surf_out) {  // every refusal of the arrays before anything launches
+    if ((rc = check_io(in, array_in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
+    if (!easu_con || bad_flags(flags)) return FSR1_ERR_INVALID_ARGUMENT;
+    if ((rc = array_rules(in, out, easu_con, flags, false)) != FSR1_OK) return rc;
   }
   if (flags & FSR1_FLAG_NO_RCAS) return easu(in, out, easu_con, y0, y1, flags, stream, sync, sync_taken);
   const Rows e = easu_rows(y0, y1, out->height);
   if ((flags & FSR1_FLAG_FUSED) && in && easu_con && rcas_con && (in->format == FSR1_FORMAT_RGBA16F || r11) &&
       out->format == FSR1_FORMAT_RGBA16F && !(flags & kNotFused)) {
-    if ((rc = check_io(in, surf_in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
-    if (flags & ~kAllFlags) return FSR1_ERR_INVALID_ARGUMENT;
+    if ((rc = check_io(in, array_in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
+    if (bad_flags(flags)) return FSR1_ERR_INVALID_ARGUMENT;
     if (y0 >= y1 || y1 > out->height) return FSR1_ERR_INVALID_ARGUMENT;
     if (!window_holds(out, (int)y0, (int)y1 - 1)) return FSR1_ERR_WINDOW;
     uint32_t r0, r1;
@@ -404,10 +449,10 @@ int upscale(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, 
   flags &= ~(uint32_t)FSR1_FLAG_FUSED;
   if (!tmp) return FSR1_ERR_INVALID_ARGUMENT;
   if (surf_out && (((uintptr_t)tmp->data & 15) || (tmp->pitch_bytes & 15))) return FSR1_ERR_UNSUPPORTED;  // the packed RCAS kernel's loads
-  // the output square and OUT_SURFACE belong to the last pass, SRTM_INPUT and IN_SURFACE to EASU's load stage
+  // the output square and OUT_SURFACE belong to the last pass, SRTM_INPUT, IN_SURFACE and IN_TEXTURE to EASU's load stage
   rc = easu(in, tmp, easu_con, e.a, e.b, flags & ~(uint32_t)(FSR1_FLAG_OUTPUT_SQUARE | FSR1_FLAG_OUT_SURFACE), stream, sync, sync_taken);
   if (rc != FSR1_OK) return rc;
-  return fsr1_rcas(tmp, out, rcas_con, y0, y1, flags & ~(uint32_t)(FSR1_FLAG_SRTM_INPUT | FSR1_FLAG_IN_SURFACE), stream);
+  return fsr1_rcas(tmp, out, rcas_con, y0, y1, flags & ~(uint32_t)(FSR1_FLAG_SRTM_INPUT | kArrayIn), stream);
 }
 
 int upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* out, const uint32_t easu_con[16],
@@ -416,8 +461,8 @@ int upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
   if (!post || post->ops == 0) return upscale(in, tmp, out, easu_con, rcas_con, y0, y1, flags, stream, sync, sync_taken);
   NvtxRange range("FSR1 upscale post");
   int rc;
-  const bool surf_in = (flags & FSR1_FLAG_IN_SURFACE) != 0, surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
-  if ((rc = check_io(in, surf_in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
+  const bool array_in = (flags & kArrayIn) != 0, surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
+  if ((rc = check_io(in, array_in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
   if (!easu_con || !rcas_con) return FSR1_ERR_INVALID_ARGUMENT;
   PostParams q;
   if ((rc = post_params(post, in->format, out->format, flags, q)) != FSR1_OK) return rc;
@@ -439,7 +484,7 @@ int upscale_post(const fsr1_image* in, const fsr1_image* tmp, const fsr1_image* 
     if (((uintptr_t)tmp->data & 15) || (tmp->pitch_bytes & 15)) return FSR1_ERR_UNSUPPORTED;
     if (!surf_out && overlaps(tmp, out)) return FSR1_ERR_INVALID_ARGUMENT;
   }
-  if ((surf_in || surf_out) && (rc = surface_rules(in, out, easu_con, flags, true)) != FSR1_OK) return rc;
+  if ((array_in || surf_out) && (rc = array_rules(in, out, easu_con, flags, true)) != FSR1_OK) return rc;
   if ((flags & FSR1_FLAG_FUSED) && !(flags & kNotFused)) {
     const cudaError_t err = launch_fused(in, out, easu_con, rcas_con, &q, y0, y1, flags, stream, sync, sync_taken);
     if (err == cudaSuccess) return FSR1_OK;
@@ -520,9 +565,9 @@ int fsr1_rcas(const fsr1_image* in, const fsr1_image* out, const uint32_t con[4]
   int rc;
   const bool surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
   if ((rc = check_image(in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
-  if (!con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
+  if (!con || bad_flags(flags)) return FSR1_ERR_INVALID_ARGUMENT;
   if (flags & FSR1_FLAG_SRTM_INPUT) return FSR1_ERR_INVALID_ARGUMENT;  // RCAS has no input stage
-  if (flags & FSR1_FLAG_IN_SURFACE) return FSR1_ERR_UNSUPPORTED;      // RCAS reads the linear intermediate
+  if (flags & kArrayIn) return FSR1_ERR_UNSUPPORTED;                   // RCAS reads the linear intermediate
   if (surf_out && ((flags & kSurfRefused) || out->format != FSR1_FORMAT_RGBA16F)) return FSR1_ERR_UNSUPPORTED;
   if (in->format != out->format || in->format == FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
   if ((rc = rcas_images(in, out, y0, y1, surf_out)) != FSR1_OK) return rc;
@@ -580,11 +625,11 @@ int fsr1_rcas_post(const fsr1_image* in, const fsr1_image* out, const uint32_t r
   NvtxRange range("RCAS post");
   // the other arithmetic paths, EASU-only frames and input surfaces: only the packed RGBA16F kernel has the input stage
   constexpr uint32_t kRefused = FSR1_FLAG_EXACT | FSR1_FLAG_FORCE_DIRECT | FSR1_FLAG_H_REFERENCE | FSR1_FLAG_PRECISE | FSR1_FLAG_RCAS_HX2 |
-                                FSR1_FLAG_NO_RCAS | FSR1_FLAG_IN_SURFACE;
+                                FSR1_FLAG_NO_RCAS | kArrayIn;
   int rc;
   const bool surf_out = (flags & FSR1_FLAG_OUT_SURFACE) != 0;
   if ((rc = check_image(in)) != FSR1_OK || (rc = check_io(out, surf_out)) != FSR1_OK) return rc;
-  if (!rcas_con || (flags & ~kAllFlags)) return FSR1_ERR_INVALID_ARGUMENT;
+  if (!rcas_con || bad_flags(flags)) return FSR1_ERR_INVALID_ARGUMENT;
   if (flags & kRefused) return FSR1_ERR_UNSUPPORTED;
   if (in->format != FSR1_FORMAT_RGBA16F && in->format != FSR1_FORMAT_R11G11B10_FLOAT) return FSR1_ERR_UNSUPPORTED;
   const bool ops = post && post->ops;
@@ -724,7 +769,7 @@ int fsr1_context_upscale(fsr1_context* c, const void* in_dev, uint64_t in_pitch,
 int fsr1_context_upscale_host(fsr1_context* c, const void* in_host, uint64_t in_pitch, void* out_host,
                               uint64_t out_pitch, float sharpness, uint32_t flags, void* stream) {
   if (!c || !in_host || !out_host) return FSR1_ERR_INVALID_ARGUMENT;
-  if (flags & kSurfFlags) return FSR1_ERR_UNSUPPORTED;  // its frames are host memory, staged through the context's linear buffers
+  if (flags & kArrayFlags) return FSR1_ERR_UNSUPPORTED;  // its frames are host memory, staged through the context's linear buffers
   const uint64_t bpp = (uint64_t)bytes_per_pixel(c->format), obpp = (uint64_t)bytes_per_pixel(easu_out_format(c->format));
   if (in_pitch < c->in_w * bpp || out_pitch < c->out_w * obpp) return FSR1_ERR_INVALID_ARGUMENT;
   cudaError_t e;

@@ -284,6 +284,37 @@ __device__ __forceinline__ void surf_store4(unsigned long long s, int x, int y, 
 }
 #endif
 
+// ---- texture access (FSR1_FLAG_IN_TEXTURE) -----------------------------------------------------------------------------------
+// A texture image's ImgView holds the cudaTextureObject_t in `base` (pitch 0, row0 0, rows = h).  The array's channels are unsigned
+// integers (16,16,16,16 for RGBA16F, 32 for R11G11B10F) read in element mode with point filtering and unnormalized coordinates, so a
+// fetch returns the texel's raw bits; the texel centre x + 0.5 is the sample position.  Callers clamp to the logical image, so the
+// address mode never applies.  tests/emu supplies these under FSR1_CPU_EMU (fsr1_emu_tex.h).
+#ifdef FSR1_CPU_EMU
+}  // namespace fsr1
+#include "fsr1_emu_tex.h"
+namespace fsr1 {
+#else
+__device__ __forceinline__ uint2 tex_load8(unsigned long long t, int x, int y) {
+  const ushort4 v = tex2D<ushort4>(t, (float)x + 0.5f, (float)y + 0.5f);
+  return make_uint2((uint32_t)v.x | ((uint32_t)v.y << 16), (uint32_t)v.z | ((uint32_t)v.w << 16));
+}
+__device__ __forceinline__ uint32_t tex_load4(unsigned long long t, int x, int y) {
+  return tex2D<unsigned int>(t, (float)x + 0.5f, (float)y + 0.5f);
+}
+#endif
+
+// Where EASU's load stage reads the input from: a TMA tensor map over linear memory, or a CUDA array whose handle is ImgView::base,
+// through a surface object (FSR1_FLAG_IN_SURFACE, RGBA16F) or a texture object (FSR1_FLAG_IN_TEXTURE, RGBA16F or R11G11B10F).
+enum InSrc : int { kInTma = 0, kInSurf = 1, kInTex = 2 };
+// The RGBA16F bits of an array input's texel at (x, y), which the caller clamped to the logical image: phase 1 of the array kernels.
+template <int kIn, bool kR11>
+__device__ __forceinline__ uint2 array_texel(unsigned long long h, int x, int y) {
+  static_assert(kIn == kInTex || (kIn == kInSurf && !kR11), "surfaces carry RGBA16F only");
+  if constexpr (kIn == kInSurf) return surf_load8(h, x, y);
+  else if constexpr (kR11) return r11_to_half(tex_load4(h, x, y));
+  else return tex_load8(h, x, y);
+}
+
 // ---- host helpers of the dispatch layer (fsr1_capi.cu, fsr1_shard.cu) -----------------------------------------------------
 inline int bytes_per_pixel(uint32_t fmt) {  // 0: not a format include/fsr1_b200.h defines
   switch (fmt) {
@@ -325,17 +356,18 @@ cudaError_t launch_rcas_direct(const RcasParams& p, int format, bool exact, cuda
 // meet their alignment needs (the caller then falls back to the direct kernels).  srtm_in: FSR1_FLAG_SRTM_INPUT (the caller
 // must not fall back then: no other kernel applies it).
 // r11: the input is R11G11B10_FLOAT (the output RGBA16F); no fall-back either (launch_easu_direct decodes the format itself).
-// surf_in (FSR1_FLAG_IN_SURFACE): p.in.base is a surface object on an RGBA16F array; surf_out (FSR1_FLAG_OUT_SURFACE): p.out.base is one.
-// No fall-back for either: no other kernel reads or writes a surface.
+// in: kInSurf (FSR1_FLAG_IN_SURFACE), p.in.base is a surface object on an RGBA16F array; kInTex (FSR1_FLAG_IN_TEXTURE), a texture object
+// on an RGBA16F or (r11) R11G11B10F array.  surf_out (FSR1_FLAG_OUT_SURFACE): p.out.base is a surface object.  No fall-back for any of
+// them: no other kernel reads an array or writes a surface.
 cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in = false, bool r11 = false,
-                                bool surf_in = false);
+                                InSrc in = kInTma);
 cudaError_t launch_rcas_h_packed(const RcasParams& p, cudaStream_t s, const char** name, bool surf_out = false);
 // UNORM images through the TMA-tiled 2x EASU / packed RCAS kernels: cudaErrorNotSupported when not applicable
 cudaError_t launch_easu_u_tiled(const EasuParams& p, int format, cudaStream_t s, const char** name);
 cudaError_t launch_rcas_u_packed(const RcasParams& p, int format, cudaStream_t s, const char** name);
 // EASU -> RCAS in one kernel (RGBA16F, exactly 2x, out-of-image taps read 0): e.in = input, e.out = final output, rows [e.y0, e.y1)
 cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in = false,
-                           bool r11 = false, bool surf_in = false, bool surf_out = false);
+                           bool r11 = false, InSrc in = kInTma, bool surf_out = false);
 cudaError_t launch_easu_f32_tiled(const EasuParams& p, cudaStream_t s, const char** name);  // RGBA32F, exactly 2x
 cudaError_t launch_easu_h_precise(const EasuParams& p, cudaStream_t s, const char** name);  // RGBA16F io, fp32 math, 2x
 cudaError_t launch_rcas_f32_packed(const RcasParams& p, cudaStream_t s, const char** name);

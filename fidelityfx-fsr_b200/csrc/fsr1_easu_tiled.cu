@@ -25,6 +25,8 @@
 //   easu_u_quad2x_kernel  the same for R8G8B8A8_UNORM images (4-byte texels, decode pass, fused re-encode).
 //   easu_h_pairs_kernel   any other scale >= 1; 64x32 output tile per CTA; lane = one output column and a VERTICAL
 //                         pixel pair.
+// Array inputs (FSR1_FLAG_IN_SURFACE / IN_TEXTURE): a TMA tensor map addresses global memory only, so the *_surf_in / *_tex_in twins
+// fill the same half tile in phase 1 from the array (array_texel, fsr1_common.cuh); the rest of each kernel is the linear one.
 // kSrtmIn (FSR1_FLAG_SRTM_INPUT, RGBA16F kernels): phase 1 first replaces each box texel by FsrSrtmF of it, rounded to half
 // (srtm_texel, fsr1_post.cuh), and takes the luma from that half texel; the taps then read the transformed tile.  It runs after
 // clamp_fixup, on the raw texels the fixup copied, so each texel is transformed once.  Its generic-proxy stores into the TMA buffer
@@ -150,12 +152,14 @@ __host__ __device__ inline size_t pairs_smem_bytes(int BW, int BH) {
 // kR11: R11G11B10_FLOAT input (fsr1_r11.cuh): the box is BW4 = BW + 2 or + 4 texels wide (a multiple of 4), from the multiple of 4 at or
 // before the half tile's origin.  BW * BH <= kR11Per * kThreads holds for every upscale (BW <= 68, BH <= 35; the launcher checks).
 constexpr int kR11Per = 10;
-// kSurfIn (FSR1_FLAG_IN_SURFACE): p.in.base is a surface object on an RGBA16F array and `tmap` is unused; phase 1 reads the box with
-// surface loads at coordinates clamped to the logical image (the texels TMA + clamp_fixup leave in it) into tile buffer 0.
-template <bool kSrtmIn = false, bool kR11 = false, bool kSurfIn = false>
+// kIn != kInTma (FSR1_FLAG_IN_SURFACE / IN_TEXTURE): p.in.base is a surface or texture object on a CUDA array and `tmap` is unused;
+// phase 1 reads the box with surface loads or texture fetches (array_texel) at coordinates clamped to the logical image (the texels
+// TMA + clamp_fixup leave in it) into tile buffer 0.  (kInSurf is 1: the surface twins are still easu_h_pairs_kernel<k, false, 1>.)
+template <bool kSrtmIn = false, bool kR11 = false, int kIn = kInTma>
 __global__ void __launch_bounds__(kThreads, 3)
 easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap, const int BW, const int BH,
                     const int tiles_x, const int n_tiles) {
+  constexpr bool kArrayIn = kIn != kInTma;  // no TMA, no mbarrier, no prefetch
 #ifdef FSR1_CPU_EMU
   unsigned char* smem_raw = fsr1_emu_dynamic_smem();
 #else
@@ -170,7 +174,7 @@ easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap
   uint64_t* bar = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(S) +
                                               (((size_t)(BW - 2) * (BH - 2) * 16 + 127) & ~(size_t)127));
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (!kSurfIn) {
+  if (!kArrayIn) {
     if (tid == 0) {
       mbar_init(&bar[0], 1);
       mbar_init(&bar[1], 1);
@@ -191,15 +195,15 @@ easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap
     fy0 -= 1;
   };
   int t = blockIdx.x;
-  if (!kSurfIn && tid == 0 && t < n_tiles) {
+  if (!kArrayIn && tid == 0 && t < n_tiles) {
     int a, b, fx, fy;
     origin(t, a, b, fx, fy);
     mbar_expect_tx(&bar[0], kR11 ? (uint32_t)(((BW + 5) & ~3) * BH) * 4u : (uint32_t)n * 8u);
     tma_load_2d(base, &tmap, kR11 ? fx & ~3 : fx, fy - p.in.row0, &bar[0]);
   }
   for (int it = 0; t < n_tiles; t += gridDim.x, it++) {
-  const int bsel = kSurfIn ? 0 : it & 1;
-  if (!kSurfIn && tid == 0 && t + (int)gridDim.x < n_tiles) {  // prefetch the next tile into the other buffer
+  const int bsel = kArrayIn ? 0 : it & 1;
+  if (!kArrayIn && tid == 0 && t + (int)gridDim.x < n_tiles) {  // prefetch the next tile into the other buffer
     int a, b, fx, fy;
     origin(t + gridDim.x, a, b, fx, fy);
     fence_proxy_async();
@@ -209,7 +213,7 @@ easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap
   uint2* tile = reinterpret_cast<uint2*>(base + bsel * tstride);
   int ox0, oy0, fx0, fy0;
   origin(t, ox0, oy0, fx0, fy0);
-  if (!kSurfIn) {
+  if (!kArrayIn) {
     mbar_wait(&bar[bsel], (it >> 1) & 1);
     if (fx0 < 0 || fy0 < 0 || fx0 + BW > p.in.w || fy0 + BH > p.in.h) {  // border tiles only (CTA-uniform)
       if constexpr (kR11) clamp_fixup(reinterpret_cast<uint32_t*>(tile) + (fx0 & 3), (BW + 5) & ~3, BW, BH, fx0, fy0, p.in.w, p.in.h, lane, warp, kThreads / 32);
@@ -219,12 +223,12 @@ easu_h_pairs_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap
     }
   }
 
-  if constexpr (kSurfIn) {  // phase 1 from the surface, row and column stepped as phase 2 steps them
+  if constexpr (kArrayIn) {  // phase 1 from the array, row and column stepped as phase 2 steps them
     const unsigned long long src = surf_of(p.in);
     int j = tid / BW, c = tid - j * BW;
     const int dj = kThreads / BW, dc = kThreads - dj * BW;
     for (int i = tid; i < n; i += kThreads) {
-      uint2 v = surf_load8(src, clampi(fx0 + c, 0, p.in.w - 1), clampi(fy0 + j, 0, p.in.h - 1));
+      uint2 v = array_texel<kIn, kR11>(src, clampi(fx0 + c, 0, p.in.w - 1), clampi(fy0 + j, 0, p.in.h - 1));
       if (kSrtmIn) v = srtm_texel(v);
       tile[i] = v;
       L[i] = texel_luma(v);
@@ -303,25 +307,26 @@ template <int NW> struct __align__(128) QuadSmem {
 
 // kR11: R11G11B10_FLOAT input (fsr1_r11.cuh): a kUBW = 40 texel box from 2 texels left of the half tile's origin (32 tx - 4: 16 bytes)
 constexpr int kUBW = kQBW + 4;
-// kSurfIn (FSR1_FLAG_IN_SURFACE): p.in.base is a surface object on an RGBA16F array and `tmap` is unused; phase 1 reads the box with
-// surface loads at coordinates clamped to the logical image (the texels TMA + clamp_fixup leave in it) into one tile buffer, which
-// the previous tile's closing barrier frees: no TMA, no mbarrier, no prefetch.
-template <int NW, bool kSrtmIn, bool kR11, bool kSurfIn = false>
+// kIn != kInTma (FSR1_FLAG_IN_SURFACE / IN_TEXTURE): p.in.base is a surface or texture object on a CUDA array and `tmap` is unused;
+// phase 1 reads the box with surface loads or texture fetches (array_texel) at coordinates clamped to the logical image (the texels
+// TMA + clamp_fixup leave in it) into one tile buffer, which the previous tile's closing barrier frees: no TMA, no mbarrier, no prefetch.
+template <int NW, bool kSrtmIn, bool kR11, int kIn = kInTma>
 __device__ __forceinline__ void quad_body(const EasuParams p, const CUtensorMap& tmap, const int tiles_x, const int n_tiles,
                                           const int mbase) {
+  constexpr bool kArrayIn = kIn != kInTma;
   using C = QuadCfg<NW>;
   constexpr int NT = NW * 32;
   constexpr uint32_t kBoxBytes = kR11 ? kUBW * C::kBH * 4u : C::kElems * 8u;
   constexpr int kShift = kR11 ? 2 : 0;
   constexpr int kStage = ((kUBW * C::kBH * 4 + 127) / 128) * 128 / 4;
   __shared__ QuadSmem<NW> sm;
-  uint32_t* stage = nullptr;  // kR11: where the boxes land (fsr1_r11.cuh)
-  if constexpr (kR11) {
+  uint32_t* stage = nullptr;  // kR11 by TMA: where the boxes land (fsr1_r11.cuh)
+  if constexpr (kR11 && !kArrayIn) {
     __shared__ R11Stage<kStage> r11_stage;
     stage = &r11_stage.w[0][0];
   }
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (!kSurfIn) {
+  if (!kArrayIn) {
     if (tid == 0) {
       mbar_init(&sm.bar[0], 1);
       mbar_init(&sm.bar[1], 1);
@@ -335,7 +340,7 @@ __device__ __forceinline__ void quad_body(const EasuParams p, const CUtensorMap&
   int t = blockIdx.x;
   int tx = t % tiles_x, ty = t / tiles_x;
   const int step_x = (int)gridDim.x % tiles_x, step_y = (int)gridDim.x / tiles_x;
-  if (!kSurfIn && tid == 0 && t < n_tiles) {
+  if (!kArrayIn && tid == 0 && t < n_tiles) {
     mbar_expect_tx(&sm.bar[0], kBoxBytes);
     tma_load_2d(kR11 ? (void*)stage : (void*)sm.tile[0], &tmap, tx * kQCX - 2 - kShift, mbase + ty * C::kCY - 1 - p.in.row0, &sm.bar[0]);
   }
@@ -343,17 +348,17 @@ __device__ __forceinline__ void quad_body(const EasuParams p, const CUtensorMap&
     const int b = it & 1;
     int txn = tx + step_x, tyn = ty + step_y;  // coordinates of the CTA's next tile
     if (txn >= tiles_x) { txn -= tiles_x; tyn++; }
-    if (!kSurfIn && tid == 0 && t + (int)gridDim.x < n_tiles) {  // prefetch it into the other buffer (its readers all passed
+    if (!kArrayIn && tid == 0 && t + (int)gridDim.x < n_tiles) {  // prefetch it into the other buffer (its readers all passed
       fence_proxy_async();                                       // the barrier that closed the previous iteration)
       mbar_expect_tx(&sm.bar[b ^ 1], kBoxBytes);
       tma_load_2d(kR11 ? (void*)(stage + (b ^ 1) * kStage) : (void*)sm.tile[b ^ 1], &tmap, txn * kQCX - 2 - kShift,
                   mbase + tyn * C::kCY - 1 - p.in.row0, &sm.bar[b ^ 1]);
     }
-    uint2* tile = sm.tile[kR11 || kSurfIn ? 0 : b];  // kR11, kSurfIn: phase 1 writes the half tile after the previous tile's closing barrier
+    uint2* tile = sm.tile[kR11 || kArrayIn ? 0 : b];  // kR11, kArrayIn: phase 1 writes the half tile after the previous tile's closing barrier
     const int gx0 = tx * kQCX - 2, gy0 = mbase + ty * C::kCY - 1;
     tx = txn;
     ty = tyn;
-    if (!kSurfIn) {
+    if (!kArrayIn) {
       mbar_wait(&sm.bar[b], (it >> 1) & 1);
       if (gx0 < 0 || gy0 < 0 || gx0 + kQBW > p.in.w || gy0 + C::kBH > p.in.h) {
         if constexpr (kR11) clamp_fixup(stage + b * kStage + kShift, kUBW, kQBW, C::kBH, gx0, gy0, p.in.w, p.in.h, lane, warp, NW);
@@ -362,11 +367,11 @@ __device__ __forceinline__ void quad_body(const EasuParams p, const CUtensorMap&
         __syncthreads();
       }
     }
-    if constexpr (kSurfIn) {
+    if constexpr (kArrayIn) {
       const unsigned long long src = surf_of(p.in);
       for (int i = tid; i < C::kElems; i += NT) {
         const int j = i / kQBW, c = i - j * kQBW;
-        uint2 v = surf_load8(src, clampi(gx0 + c, 0, p.in.w - 1), clampi(gy0 + j, 0, p.in.h - 1));
+        uint2 v = array_texel<kIn, kR11>(src, clampi(gx0 + c, 0, p.in.w - 1), clampi(gy0 + j, 0, p.in.h - 1));
         if (kSrtmIn) v = srtm_texel(v);
         tile[i] = v;
         sm.L[i] = texel_luma(v);
@@ -413,7 +418,14 @@ template <int NW, int MINB, bool kSrtmIn>
 __global__ void __launch_bounds__(NW * 32, MINB)
 easu_h_quad2x_surf_in_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap, const int tiles_x, const int n_tiles,
                              const int mbase) {
-  quad_body<NW, kSrtmIn, false, true>(p, tmap, tiles_x, n_tiles, mbase);
+  quad_body<NW, kSrtmIn, false, kInSurf>(p, tmap, tiles_x, n_tiles, mbase);
+}
+// FSR1_FLAG_IN_TEXTURE: the RGBA16F or (kR11) R11G11B10F kernel reading its input through a texture object (`tmap` unused)
+template <int NW, int MINB, bool kSrtmIn, bool kR11>
+__global__ void __launch_bounds__(NW * 32, MINB)
+easu_h_quad2x_tex_in_kernel(const EasuParams p, const __grid_constant__ CUtensorMap tmap, const int tiles_x, const int n_tiles,
+                            const int mbase) {
+  quad_body<NW, kSrtmIn, kR11, kInTex>(p, tmap, tiles_x, n_tiles, mbase);
 }
 template <int NW, int MINB, bool kSrtmIn>
 __global__ void __launch_bounds__(NW * 32, MINB)
@@ -566,13 +578,14 @@ cudaError_t launch_easu_u_tiled(const EasuParams& p, int format, cudaStream_t s,
   return cudaGetLastError();
 }
 
-cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in, bool r11, bool surf_in) {
+cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char** name, bool srtm_in, bool r11, InSrc in) {
+  const bool surf_in = in == kInSurf, tex_in = in == kInTex, array_in = in != kInTma;
   // layout requirements of TMA and of the vector stores
-  if ((!surf_in && ((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15))) || (reinterpret_cast<uintptr_t>(p.out.base) & 15) ||
+  if ((!array_in && ((reinterpret_cast<uintptr_t>(p.in.base) & 15) || (p.in.pitch & 15))) || (reinterpret_cast<uintptr_t>(p.out.base) & 15) ||
       (p.out.pitch & 15))
     return cudaErrorNotSupported;
   CUtensorMap tmap;
-  if (surf_in) memset(&tmap, 0, sizeof tmap);  // read by no kernel: the input is a surface object
+  if (array_in) memset(&tmap, 0, sizeof tmap);  // read by no kernel: the input is a surface or texture object
   const CUtensorMapDataType type = r11 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT64;
 
   if (is_2x(p.c0x, p.c0y, p.c0z, p.c0w)) {
@@ -581,9 +594,16 @@ cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char*
     // registers are taken but 256, so the one-warp halo_push_kernel that the wait depends on cannot be placed beside a
     // grid that fills every SM, and ranks sharing one GPU would wait for each other until the spin timeout.
     constexpr int NW = 4, CY = 2 * NW;
-    if (!surf_in && !make_tmap(&tmap, p.in, r11 ? kUBW : kQBW, CY + 3, type)) return cudaErrorNotSupported;
+    if (!array_in && !make_tmap(&tmap, p.in, r11 ? kUBW : kQBW, CY + 3, type)) return cudaErrorNotSupported;
     const QuadGrid g = quad_grid(p, CY, (p.sync.ready[0] || p.sync.ready[1]) ? 6 : 7);
-    if (surf_in) {
+    if (tex_in) {
+      if (r11 && srtm_in) easu_h_quad2x_tex_in_kernel<NW, 7, true, true><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
+      else if (r11) easu_h_quad2x_tex_in_kernel<NW, 7, false, true><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
+      else if (srtm_in) easu_h_quad2x_tex_in_kernel<NW, 7, true, false><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
+      else easu_h_quad2x_tex_in_kernel<NW, 7, false, false><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
+      *name = r11 ? (srtm_in ? "easu_h_quad2x<4w,7/sm,r11g11b10f_in,srtm_in,tex_in>" : "easu_h_quad2x<4w,7/sm,r11g11b10f_in,tex_in>")
+                  : (srtm_in ? "easu_h_quad2x<4w,7/sm,srtm_in,tex_in>" : "easu_h_quad2x<4w,7/sm,tex_in>");
+    } else if (surf_in) {
       if (srtm_in) easu_h_quad2x_surf_in_kernel<NW, 7, true><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
       else easu_h_quad2x_surf_in_kernel<NW, 7, false><<<g.grid, NW * 32, 0, s>>>(p, tmap, g.tiles_x, g.n_tiles, g.m_first);
       *name = srtm_in ? "easu_h_quad2x<4w,7/sm,srtm_in,surf_in>" : "easu_h_quad2x<4w,7/sm,surf_in>";
@@ -611,9 +631,11 @@ cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char*
   if (r11 && BW * BH > kR11Per * kThreads) return cudaErrorNotSupported;  // cannot happen when upscaling (pairs_body)
   const size_t smem = pairs_smem_bytes(BW, BH);
   if (smem > 200 * 1024) return cudaErrorNotSupported;
-  if (!surf_in && !make_tmap(&tmap, p.in, r11 ? (BW + 5) & ~3 : BW, BH, type)) return cudaErrorNotSupported;
+  if (!array_in && !make_tmap(&tmap, p.in, r11 ? (BW + 5) & ~3 : BW, BH, type)) return cudaErrorNotSupported;
   void (*kernel)(const EasuParams, const CUtensorMap, const int, const int, const int, const int) =
-      surf_in ? (srtm_in ? easu_h_pairs_kernel<true, false, true> : easu_h_pairs_kernel<false, false, true>)
+      tex_in  ? (r11 ? (srtm_in ? easu_h_pairs_kernel<true, true, kInTex> : easu_h_pairs_kernel<false, true, kInTex>)
+                     : (srtm_in ? easu_h_pairs_kernel<true, false, kInTex> : easu_h_pairs_kernel<false, false, kInTex>))
+      : surf_in ? (srtm_in ? easu_h_pairs_kernel<true, false, kInSurf> : easu_h_pairs_kernel<false, false, kInSurf>)
       : r11   ? (srtm_in ? easu_h_pairs_kernel<true, true> : easu_h_pairs_kernel<false, true>)
               : (srtm_in ? easu_h_pairs_kernel<true, false> : easu_h_pairs_kernel<false, false>);
   if (smem > 48 * 1024) {  // per device and cheap: set on every launch that needs the opt-in
@@ -625,7 +647,9 @@ cudaError_t launch_easu_h_tiled(const EasuParams& p, cudaStream_t s, const char*
   while (per_sm > 1 && (size_t)per_sm * (smem + 1024) > 220 * 1024) per_sm--;
   const int grid = n_tiles < per_sm * sm_count() ? n_tiles : per_sm * sm_count();
   kernel<<<grid, kThreads, smem, s>>>(p, tmap, BW, BH, tiles_x, n_tiles);
-  *name = surf_in ? (srtm_in ? "easu_h_vpairs<64x32,persistent,srtm_in,surf_in>" : "easu_h_vpairs<64x32,persistent,surf_in>")
+  *name = tex_in  ? (r11 ? (srtm_in ? "easu_h_vpairs<64x32,persistent,r11g11b10f_in,srtm_in,tex_in>" : "easu_h_vpairs<64x32,persistent,r11g11b10f_in,tex_in>")
+                         : (srtm_in ? "easu_h_vpairs<64x32,persistent,srtm_in,tex_in>" : "easu_h_vpairs<64x32,persistent,tex_in>"))
+          : surf_in ? (srtm_in ? "easu_h_vpairs<64x32,persistent,srtm_in,surf_in>" : "easu_h_vpairs<64x32,persistent,surf_in>")
           : r11   ? (srtm_in ? "easu_h_vpairs<64x32,persistent,tma2,r11g11b10f_in,srtm_in>" : "easu_h_vpairs<64x32,persistent,tma2,r11g11b10f_in>")
                   : (srtm_in ? "easu_h_vpairs<64x32,persistent,tma2,srtm_in>" : "easu_h_vpairs<64x32,persistent,tma2>");
   return cudaGetLastError();

@@ -30,6 +30,8 @@
 // TMA load into the buffer orders the stores).  Those kFBW (n + 3) texels are exactly the ones the step's taps read.
 // kR11 (R11G11B10_FLOAT input, fsr1_r11.cuh): a kRBW = 40 texel box of 4-byte texels from the multiple of 4 at or before box_x (38
 // texels are 152 bytes: TMA boxes are multiples of 16 bytes), expanded in phase 1 into the same half tile, the step's kFBW (n + 3) texels.
+// Array inputs (FSR1_FLAG_IN_SURFACE: RGBA16F; FSR1_FLAG_IN_TEXTURE: RGBA16F or R11G11B10F): phase 1 fetches the step's texels from the
+// CUDA array at clamped coordinates instead (fused_body's kIn); the *_surf and *_tex kernels below.
 #include "fsr1_easu_quad.cuh"
 #include "fsr1_post.cuh"
 #include "fsr1_r11.cuh"
@@ -233,23 +235,25 @@ __device__ __forceinline__ void fused_step(FusedSmem<NW>& sm, const FusedParams&
   }
 }
 
-// kSurfIn (FSR1_FLAG_IN_SURFACE): p.in.base is a surface object on an RGBA16F array and `tmap` is unused.  Phase 1 reads the step's
-// kFBW (n + 3) texels with surface loads at coordinates clamped to the logical image (the texels TMA + clamp_fixup would leave in the
-// tile), into one tile buffer: no TMA, no mbarrier, no prefetch.  The previous step's closing barrier frees the buffer.
-template <int NW, typename SO, bool kSrtmIn, bool kR11 = false, bool kSurfIn = false, bool kSurfOut = false>
+// kIn != kInTma (FSR1_FLAG_IN_SURFACE / IN_TEXTURE): p.in.base is a surface or texture object on a CUDA array and `tmap` is unused.
+// Phase 1 reads the step's kFBW (n + 3) texels with surface loads or texture fetches (array_texel) at coordinates clamped to the
+// logical image (the texels TMA + clamp_fixup would leave in the tile), into one tile buffer: no TMA, no mbarrier, no prefetch.  The
+// previous step's closing barrier frees the buffer.  (kInSurf is 1, so the surface twins' bool kSurfIn selects it.)
+template <int NW, typename SO, bool kSrtmIn, bool kR11 = false, int kIn = kInTma, bool kSurfOut = false>
 __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMap& tmap, const PostParams* q) {
+  constexpr bool kArrayIn = kIn != kInTma;
   using C = FusedCfg<NW>;
   constexpr int NT = NW * 32, CY = C::kCY;
   constexpr uint32_t kBoxBytes = kR11 ? kRBW * C::kBH * 4u : C::kElems * 8u;
   constexpr int kStage = ((kRBW * C::kBH * 4 + 127) / 128) * 128 / 4;
   __shared__ FusedSmem<NW> sm;
-  uint32_t* stage = nullptr;  // kR11: where the boxes land (fsr1_r11.cuh)
-  if constexpr (kR11) {
+  uint32_t* stage = nullptr;  // kR11 by TMA: where the boxes land (fsr1_r11.cuh)
+  if constexpr (kR11 && !kArrayIn) {
     __shared__ R11Stage<kStage> r11_stage;
     stage = &r11_stage.w[0][0];
   }
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (!kSurfIn) {
+  if (!kArrayIn) {
     if (tid == 0) {
       mbar_init(&sm.bar[0], 1);
       mbar_init(&sm.bar[1], 1);
@@ -264,7 +268,7 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
   bool has = iter.next(cur);
   auto box_x = [](const FusedStep& s) { return (kStripCells * s.tx - 2) & ~1; };  // even texel at or before the first tap column
   auto tma_x = [&](const FusedStep& s) { return kR11 ? box_x(s) & ~3 : box_x(s); };
-  if (!kSurfIn && tid == 0 && has) {
+  if (!kArrayIn && tid == 0 && has) {
     mbar_expect_tx(&sm.bar[0], kBoxBytes);
     tma_load_2d(kR11 ? (void*)stage : (void*)sm.tile[0], &tmap, tma_x(cur), cur.m0 - 1 - p.in.row0, &sm.bar[0]);
   }
@@ -272,17 +276,17 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
   for (int it = 0; has; it++) {
     const int b = it & 1;
     const bool hasn = iter.next(nxt);
-    if (!kSurfIn && tid == 0 && hasn) {  // prefetch the next step's box into the other buffer (its readers passed the closing barrier)
+    if (!kArrayIn && tid == 0 && hasn) {  // prefetch the next step's box into the other buffer (its readers passed the closing barrier)
       fence_proxy_async();
       mbar_expect_tx(&sm.bar[b ^ 1], kBoxBytes);
       tma_load_2d(kR11 ? (void*)(stage + (b ^ 1) * kStage) : (void*)sm.tile[b ^ 1], &tmap, tma_x(nxt), nxt.m0 - 1 - p.in.row0,
                   &sm.bar[b ^ 1]);
     }
-    uint2* tile = sm.tile[kR11 || kSurfIn ? 0 : b];  // kR11, kSurfIn: phase 1 writes the half tile after the previous step's closing barrier
+    uint2* tile = sm.tile[kR11 || kArrayIn ? 0 : b];  // kR11, kArrayIn: phase 1 writes the half tile after the previous step's closing barrier
     const int k0 = kStripCells * cur.tx - 1;       // first cell of the strip (lane 0)
     const int gxe = box_x(cur), dx = (k0 - 1) - gxe;  // box origin; offset of tap column 0 of lane 0 inside it (0 or 1)
     const int gy0 = cur.m0 - 1, n = cur.n;
-    if (!kSurfIn) {
+    if (!kArrayIn) {
       mbar_wait(&sm.bar[b], (it >> 1) & 1);
       if (gxe < 0 || gy0 < 0 || gxe + kFBW > p.in.w || gy0 + C::kBH > p.in.h) {
         if constexpr (kR11) clamp_fixup(stage + b * kStage + (gxe & 3), kRBW, kFBW, C::kBH, gxe, gy0, p.in.w, p.in.h, lane, warp, NW);
@@ -292,11 +296,11 @@ __device__ __forceinline__ void fused_body(const FusedParams p, const CUtensorMa
       }
     }
     // phases 1 and 2 on the rows this step needs (n + 3 texel rows, n + 1 rows of terms)
-    if constexpr (kSurfIn) {
+    if constexpr (kArrayIn) {
       const unsigned long long src = surf_of(p.in);
       for (int i = tid; i < kFBW * (n + 3); i += NT) {
         const int j = i / kFBW, c = i - j * kFBW;
-        uint2 t = surf_load8(src, clampi(gxe + c, 0, p.in.w - 1), clampi(gy0 + j, 0, p.in.h - 1));
+        uint2 t = array_texel<kIn, kR11>(src, clampi(gxe + c, 0, p.in.w - 1), clampi(gy0 + j, 0, p.in.h - 1));
         if (kSrtmIn) t = srtm_texel(t);
         tile[i] = t;
         sm.L[i] = texel_luma(t);
@@ -375,26 +379,39 @@ fused_h_quad2x_post_surf_kernel(const FusedParams p, const __grid_constant__ CUt
   fused_body<NW, SO, kSrtmIn, false, kSurfIn, kSurfOut>(p, tmap, &q);
 }
 
+// FSR1_FLAG_IN_TEXTURE: the same two kernels reading their RGBA16F or (kR11) R11G11B10F input through a texture object (`tmap` unused),
+// writing a linear output or with kSurfOut a surface
+template <int NW, int MINB, bool kSrtmIn, bool kR11, bool kSurfOut>
+__global__ void __launch_bounds__(NW * 32, MINB)
+fused_h_quad2x_tex_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap) {
+  fused_body<NW, void, kSrtmIn, kR11, kInTex, kSurfOut>(p, tmap, nullptr);
+}
+template <int NW, int MINB, typename SO, bool kSrtmIn, bool kR11, bool kSurfOut>
+__global__ void __launch_bounds__(NW * 32, MINB)
+fused_h_quad2x_post_tex_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmap, const __grid_constant__ PostParams q) {
+  fused_body<NW, SO, kSrtmIn, kR11, kInTex, kSurfOut>(p, tmap, &q);
+}
+
 #ifndef FSR1_CPU_EMU
 // tensor map, parameters and grid of a fused launch; cudaErrorNotSupported when the frame is not one the kernel takes.
-// out_align: the alignment the output store needs (16 for RGBA16F pairs, 8 for UNORM pairs).  surf_in / surf_out: that side is a
-// surface object (no alignment rule; no tensor map for a surface input: `tmap` is zeroed).
+// out_align: the alignment the output store needs (16 for RGBA16F pairs, 8 for UNORM pairs).  array_in / surf_out: the input is a
+// surface or texture object, the output a surface object (no alignment rule; no tensor map for an array input: `tmap` is zeroed).
 static cudaError_t fused_setup(const EasuParams& e, uint32_t sharp_h2, int out_align, bool r11, CUtensorMap& tmap, FusedParams& p,
-                               int& per_sm, long long& grid, bool surf_in = false, bool surf_out = false) {
+                               int& per_sm, long long& grid, bool array_in = false, bool surf_out = false) {
   if (!is_2x(e.c0x, e.c0y, e.c0z, e.c0w)) return cudaErrorNotSupported;
-  if ((!surf_in && ((reinterpret_cast<uintptr_t>(e.in.base) & 15) || (e.in.pitch & 15))) ||
+  if ((!array_in && ((reinterpret_cast<uintptr_t>(e.in.base) & 15) || (e.in.pitch & 15))) ||
       (!surf_out && ((reinterpret_cast<uintptr_t>(e.out.base) & (out_align - 1)) || (e.out.pitch & (out_align - 1)))))
     return cudaErrorNotSupported;
   constexpr int NW = 4;
   using C = FusedCfg<NW>;
   EncodeTiledFn encode = get_encode_fn();
-  if (surf_in) memset(&tmap, 0, sizeof tmap);
+  if (array_in) memset(&tmap, 0, sizeof tmap);
   else if (!encode) return cudaErrorNotSupported;
   const cuuint64_t dims[2] = {(cuuint64_t)e.in.w, (cuuint64_t)e.in.rows};
   const cuuint64_t strides[1] = {(cuuint64_t)e.in.pitch};
   const cuuint32_t box[2] = {(cuuint32_t)(r11 ? kRBW : kFBW), (cuuint32_t)C::kBH};
   const cuuint32_t estr[2] = {1, 1};
-  if (!surf_in &&
+  if (!array_in &&
       encode(&tmap, r11 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, e.in.base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
     return cudaErrorNotSupported;
@@ -468,15 +485,76 @@ static cudaError_t launch_surf(const FusedParams& p, const CUtensorMap& tmap, co
   return cudaGetLastError();
 }
 
+// FSR1_FLAG_IN_TEXTURE: the texture twin of the plain or post kernel, at the CTAs per SM of its surface-input twin
+template <typename SO, bool kSrtmIn, bool kR11, bool kSurfOut>
+static void tex_kernel(const FusedParams& p, const CUtensorMap& tmap, const PostParams* q, long long grid, cudaStream_t s) {
+  if constexpr (std::is_void<SO>::value)
+    fused_h_quad2x_tex_kernel<4, surf_per_sm(true, kSurfOut), kSrtmIn, kR11, kSurfOut><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
+  else fused_h_quad2x_post_tex_kernel<4, kPostPerSm, SO, kSrtmIn, kR11, kSurfOut><<<(int)grid, 4 * 32, 0, s>>>(p, tmap, *q);
+}
+// rows as kSurfNames; index within a row: (r11 ? 4 : 0) | (srtm_in ? 2 : 0) | (surf_out ? 1 : 0)
+static const char* const kTexNames[4][8] = {
+    {"fused_easu_rcas_h_quad2x<4w,7/sm,strips,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,srtm_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,srtm_in,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,r11g11b10f_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,r11g11b10f_in,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,r11g11b10f_in,srtm_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,7/sm,strips,r11g11b10f_in,srtm_in,tex_in,surf_out>"},
+    {"fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,srtm_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,srtm_in,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,r11g11b10f_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,r11g11b10f_in,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,r11g11b10f_in,srtm_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba16f,r11g11b10f_in,srtm_in,tex_in,surf_out>"},
+    {"fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,srtm_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,srtm_in,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,r11g11b10f_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,r11g11b10f_in,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,r11g11b10f_in,srtm_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgba8,r11g11b10f_in,srtm_in,tex_in,surf_out>"},
+    {"fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,srtm_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,srtm_in,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,r11g11b10f_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,r11g11b10f_in,tex_in,surf_out>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,r11g11b10f_in,srtm_in,tex_in>",
+      "fused_easu_rcas_h_quad2x<4w,6/sm,strips,post,rgb10a2,r11g11b10f_in,srtm_in,tex_in,surf_out>"}};
+template <typename SO>
+static cudaError_t launch_tex(const FusedParams& p, const CUtensorMap& tmap, const PostParams* q, long long grid, bool srtm_in, bool r11,
+                              bool surf_out, cudaStream_t s, const char** name, int names_row) {
+  const int v = (r11 ? 4 : 0) | (srtm_in ? 2 : 0) | (surf_out ? 1 : 0);
+  switch (v) {
+    case 0: tex_kernel<SO, false, false, false>(p, tmap, q, grid, s); break;
+    case 1: tex_kernel<SO, false, false, true>(p, tmap, q, grid, s); break;
+    case 2: tex_kernel<SO, true, false, false>(p, tmap, q, grid, s); break;
+    case 3: tex_kernel<SO, true, false, true>(p, tmap, q, grid, s); break;
+    case 4: tex_kernel<SO, false, true, false>(p, tmap, q, grid, s); break;
+    case 5: tex_kernel<SO, false, true, true>(p, tmap, q, grid, s); break;
+    case 6: tex_kernel<SO, true, true, false>(p, tmap, q, grid, s); break;
+    default: tex_kernel<SO, true, true, true>(p, tmap, q, grid, s); break;
+  }
+  *name = kTexNames[names_row][v];
+  return cudaGetLastError();
+}
+
 cudaError_t launch_fused_h(const EasuParams& e, uint32_t sharp_h2, int clamp, cudaStream_t s, const char** name, bool srtm_in, bool r11,
-                           bool surf_in, bool surf_out) {
+                           InSrc in, bool surf_out) {
   if (clamp) return cudaErrorNotSupported;
+  const bool surf_in = in == kInSurf;
   CUtensorMap tmap;
   FusedParams p;
-  int per_sm = surf_per_sm(surf_in, surf_out);
+  int per_sm = surf_per_sm(in != kInTma, surf_out);
   long long grid = 0;
-  const cudaError_t err = fused_setup(e, sharp_h2, 16, r11, tmap, p, per_sm, grid, surf_in, surf_out);
+  const cudaError_t err = fused_setup(e, sharp_h2, 16, r11, tmap, p, per_sm, grid, in != kInTma, surf_out);
   if (err != cudaSuccess) return err;
+  if (in == kInTex) return launch_tex<void>(p, tmap, nullptr, grid, srtm_in, r11, surf_out, s, name, 0);
   if (surf_in || surf_out) return launch_surf<void>(p, tmap, nullptr, grid, srtm_in, surf_in, surf_out, s, name, 0);  // RGBA16F input
   if (r11 && srtm_in) {
     fused_r11_quad2x_kernel<4, 7, true><<<(int)grid, 4 * 32, 0, s>>>(p, tmap);
@@ -532,14 +610,22 @@ static cudaError_t launch_post_kernel(const FusedParams& p, const CUtensorMap& t
 }
 
 cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const PostParams& q, int out_format, cudaStream_t s,
-                                const char** name, bool srtm_in, bool r11, bool surf_in, bool surf_out) {
+                                const char** name, bool srtm_in, bool r11, InSrc in, bool surf_out) {
   if (out_format != 1 && out_format != 3 && out_format != 4) return cudaErrorNotSupported;
+  const bool surf_in = in == kInSurf;
   CUtensorMap tmap;
   FusedParams p;
   int per_sm = kPostPerSm;
   long long grid = 0;
-  const cudaError_t err = fused_setup(e, sharp_h2, out_format == 1 ? 16 : 8, r11, tmap, p, per_sm, grid, surf_in, surf_out);
+  const cudaError_t err = fused_setup(e, sharp_h2, out_format == 1 ? 16 : 8, r11, tmap, p, per_sm, grid, in != kInTma, surf_out);
   if (err != cudaSuccess) return err;
+  if (in == kInTex) {
+    switch (out_format) {
+      case 1: return launch_tex<__half>(p, tmap, &q, grid, srtm_in, r11, surf_out, s, name, 1);
+      case 3: return launch_tex<Unorm8>(p, tmap, &q, grid, srtm_in, r11, surf_out, s, name, 2);
+      default: return launch_tex<Unorm10>(p, tmap, &q, grid, srtm_in, r11, surf_out, s, name, 3);
+    }
+  }
   if (surf_in || surf_out) {  // RGBA16F input
     switch (out_format) {
       case 1: return launch_surf<__half>(p, tmap, &q, grid, srtm_in, surf_in, surf_out, s, name, 1);

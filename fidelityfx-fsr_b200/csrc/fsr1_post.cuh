@@ -236,9 +236,10 @@ __device__ __forceinline__ void post_pair(const PostParams& q, const PostCursor&
 
 // launchers (fsr1_fused.cu, fsr1_rcas_packed.cu); out_format 1 RGBA16F, 3 RGBA8_UNORM, 4 RGB10A2_UNORM.  cudaErrorNotSupported: the
 // frame or layout is not one the kernel takes (nothing launched).
-// surf_in / surf_out: FSR1_FLAG_IN_SURFACE / OUT_SURFACE (e.in / p.out hold surface objects; no fall-back when declined).
+// in / surf_out: FSR1_FLAG_IN_SURFACE or IN_TEXTURE / OUT_SURFACE (e.in holds the array's surface or texture object, p.out a surface
+// object; no fall-back when declined).
 cudaError_t launch_fused_h_post(const EasuParams& e, uint32_t sharp_h2, const PostParams& q, int out_format, cudaStream_t s,
-                                const char** name, bool srtm_in = false, bool r11 = false, bool surf_in = false, bool surf_out = false);
+                                const char** name, bool srtm_in = false, bool r11 = false, InSrc in = kInTma, bool surf_out = false);
 cudaError_t launch_rcas_h_post(const RcasParams& p, const PostParams& q, int out_format, cudaStream_t s, const char** name,
                                bool surf_out = false);
 // fsr1_rcas_post's input stage: p.in is R11G11B10_FLOAT (r11, 8-byte aligned) or RGBA16F (16-byte aligned), read through FsrSrtmF with

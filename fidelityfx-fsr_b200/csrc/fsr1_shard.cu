@@ -367,7 +367,7 @@ int fsr1_shard_create_post(fsr1_shard** out_sh, uint32_t in_w, uint32_t in_h, ui
   if (!bpp || !out_bpp) return FSR1_ERR_INVALID_ARGUMENT;
   if (world > in_h || world > out_h) return FSR1_ERR_INVALID_ARGUMENT;  // no empty slabs
   // the windows are linear memory the ranks export to each other, and the slabs the shard's own
-  if (flags & (FSR1_FLAG_IN_SURFACE | FSR1_FLAG_OUT_SURFACE)) return FSR1_ERR_UNSUPPORTED;
+  if (flags & (FSR1_FLAG_IN_SURFACE | FSR1_FLAG_OUT_SURFACE | FSR1_FLAG_IN_TEXTURE)) return FSR1_ERR_UNSUPPORTED;
   // the display steps: fsr1_upscale_post's rules, before any CUDA call; without them the slabs are in the input's format
   const uint32_t post_ops = post ? post->ops : 0u;
   if (post_ops) {

@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame, fsr1_shard_create_post / fsr1_shard_post, FSR1_FORMAT_R11G11B10_FLOAT, FSR1_FLAG_IN_SURFACE / FSR1_FLAG_OUT_SURFACE, fsr1_rcas_post */
+#define FSR1_ABI_VERSION 3  /* additions that leave existing callers untouched keep the number: FSR1_FLAG_RCAS_HX2, fsr1_srtm_h / fsr1_lfga_h / fsr1_tepd_h, fsr1_upscale_post, FSR1_FLAG_SRTM_INPUT, FSR1_SHARD_DYNAMIC / fsr1_shard_frame, fsr1_shard_create_post / fsr1_shard_post, FSR1_FORMAT_R11G11B10_FLOAT, FSR1_FLAG_IN_SURFACE / FSR1_FLAG_OUT_SURFACE, fsr1_rcas_post, FSR1_FLAG_IN_TEXTURE */
 
 enum {
   FSR1_OK = 0,
@@ -111,6 +111,7 @@ enum {
                                        fsr1_rcas: FSR1_ERR_INVALID_ARGUMENT. */
   FSR1_FLAG_IN_SURFACE = 1u << 12,  /* `in` is a CUDA surface object on a 2D CUDA array (EASU's load stage); see "surface images" */
   FSR1_FLAG_OUT_SURFACE = 1u << 13, /* `out` is a CUDA surface object on a 2D CUDA array (the store of the pass that writes `out`) */
+  FSR1_FLAG_IN_TEXTURE = 1u << 14,  /* `in` is a CUDA texture object on a 2D CUDA array (EASU's load stage); see "texture images" */
   FSR1_FLAG_H_REFERENCE = 1u << 4  /* fp16 images only: the literal FsrEasuH / FsrRcasH arithmetic (packed-half
                                        algorithm, half magic numbers, per-operation half rounding), bit-identical
                                        to the reference's H source; a parity path, slower and LESS accurate than
@@ -154,6 +155,30 @@ typedef struct fsr1_image {
  * pitch other than 0 or a window), then the array behind each handle (cudaGetSurfaceObjectResourceDesc, cudaArrayGetInfo): an unknown
  * handle or an extent smaller than width x height returns FSR1_ERR_INVALID_ARGUMENT; a resource that is not a 2D array, or an element
  * size other than the format's, FSR1_ERR_UNSUPPORTED. */
+
+/* Texture images (FSR1_FLAG_IN_TEXTURE): the render target read the way the reference reads it, by sampling (an SRV), so an array
+ * mapped without surface load/store (a render target created without storage / UAV usage, or an R11G11B10_FLOAT one whose format has
+ * no storage support) is read in place.  `data` holds the cudaTextureObject_t, pitch_bytes is 0, row0 = 0 and rows = height: never a
+ * window.  width x height is the logical size, the TOP-LEFT region of the array; EASU clamps its taps at the logical edge and fetches
+ * no texel outside it.  Formats: FSR1_FORMAT_RGBA16F and FSR1_FORMAT_R11G11B10_FLOAT.  The kernels use the raw texel bits, so every
+ * result is bit-identical to the same call on a linear image holding the same pixels (NaN payloads, -0 and denormals included), and:
+ *   - the array's channels are UNSIGNED INTEGERS of the texel's layout: map RGBA16F with
+ *     cudaCreateChannelDesc(16, 16, 16, 16, cudaChannelFormatKindUnsigned) and R11G11B10_FLOAT with
+ *     cudaCreateChannelDesc(32, 0, 0, 0, cudaChannelFormatKindUnsigned) (CU_AD_FORMAT_UNSIGNED_INT16 x 4 / UNSIGNED_INT32 x 1);
+ *     a float channel kind would have the texture unit convert to fp32: FSR1_ERR_UNSUPPORTED;
+ *   - the texture description: cudaReadModeElementType, normalizedCoords 0, cudaFilterModePoint, sRGB 0; any address mode (every
+ *     fetch is inside the array);
+ *   - the resource: cudaResourceTypeArray, a 2D array (not layered, not 3D) of at least width x height; a pitch2D, linear or
+ *     mipmapped-array resource is refused (pass the level-0 array of a mipmapped one).
+ * FSR1_FLAG_IN_TEXTURE is taken exactly where FSR1_FLAG_IN_SURFACE is, with the same rules otherwise: fsr1_easu, fsr1_upscale (fused,
+ * or EASU -> tmp -> RCAS), fsr1_upscale_post (every output format, FSR1_FLAG_OUT_SURFACE too) and fsr1_context_upscale / _render /
+ * _post (`in_dev` is the handle, `in_pitch` 0), with FSR1_FLAG_SRTM_INPUT too.  FSR1_ERR_UNSUPPORTED, with nothing launched: fsr1_rcas,
+ * fsr1_rcas_post, fsr1_context_upscale_host, fsr1_shard_create and fsr1_shard_create_post with the flag, another input format,
+ * FSR1_FLAG_EXACT / FORCE_DIRECT / H_REFERENCE / PRECISE / RCAS_HX2, and constants that do not upscale.  FSR1_FLAG_IN_TEXTURE together
+ * with FSR1_FLAG_IN_SURFACE: FSR1_ERR_INVALID_ARGUMENT.  Validation, before any launch: first the flag, format and layout rules (no
+ * CUDA call), then the handle (cudaGetTextureObjectResourceDesc, cudaGetTextureObjectTextureDesc, cudaArrayGetInfo): an unknown handle
+ * or an extent smaller than width x height returns FSR1_ERR_INVALID_ARGUMENT; a wrong channel kind or size, texture description or
+ * resource type, FSR1_ERR_UNSUPPORTED. */
 
 /* EASU over output rows [y0, y1) (y1 == 0 means "to the last row").  con = con0..con3, 16 words.  in and out have the same format, but
  * for R11G11B10_FLOAT input, whose output is RGBA16F. */
